@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """bench.py -- batched L-BFGS instances/second, Rosenbrock d=128 fp64, m=10
-(BASELINE.json configs[1]), on N B200s of one node.
+(BASELINE.json configs[1]), on N H100s of one node.
 
 One "step" = one batched Solver::Minimize over B = 2^20 instances per GPU
 (x0 generated on the device by the counter-based generator of SURVEY.md 8(d),
-resident in HBM when the timed region starts; 1 GiB of x0 per GPU > 126 MB L2,
+resident in HBM when the timed region starts; 1 GiB of x0 per GPU > 50 MB L2,
 so nothing is cache-warm between steps) + the global stop test (convergence
 bitmaps, one all-gather) + the D2H read of `status` (SURVEY.md 8(d)).  Timing:
 CUDA events on the launching stream bracketed by barrier + synchronize, max
@@ -14,28 +14,19 @@ over ranks.
   e2e       the same metric through the host-buffer C-ABI call
             cno_minimize_host (pinned host x0 -> H2D -> solve -> D2H of the whole
             returned state/progress), WALL-CLOCK around the call, max over ranks
-  roofline  two yardsticks for the dominant kernel, both from THIS run's
-            iteration counts and kernel time:
-              (hbm)     ALGORITHMIC bytes of the state-streaming model
-                        (SURVEY.md 8(d): w*d*(2 k_t + 6) per iteration) against
-                        MEASURED_PEAKS.json's copy bandwidth.  The fused kernel
-                        keeps the (s, y) history on chip, so this fraction can
-                        exceed 1; `traffic` (ncu DRAM bytes per launch) shows
-                        what HBM really moved.
-              (compute) the resource that binds: the FP64 datapath.  FP64-pipe
-                        warp instructions (+ FP64 tensor-core MMAs at their
-                        measured issue cost) per solver iteration come from the
-                        ncu instruction mix committed under profiles/; achieved
-                        = that x the run's iterations / kernel time, peak =
-                        SMs x 4 sub-partitions x 0.5 FP64 warp-instr/clk x the
-                        SM clock sampled during the run.
+  roofline  ALGORITHMIC bytes of the state-streaming model (SURVEY.md 8(d):
+            w*d*(2 k_t + 6) per iteration) from THIS run's iteration counts and
+            kernel time, against MEASURED_PEAKS.json's copy bandwidth (else the
+            H100 SXM data-sheet 3.35 TB/s).  The fused kernel keeps the (s, y)
+            history on chip, so this fraction can exceed 1.
   cpu_baseline  the CPU oracle (plain-C port of the reference path, OpenMP over
             instances, every host core the process may use) on a bounded prefix
             of the same batch.
   parity    >= 256 strided instances of the TIMED batch checked against the CPU
             oracle inside this run (iteration counts, status, x* bits).
   strong    (N > 1) the same global B = 2^20 split over the N GPUs.
-  other_configs  (N = 1) BASELINE.json configs[2..4]: device timing + binding pipe.
+  other_configs  (N = 1) BASELINE.json configs[2..4]: device timing.
+--dump-outputs DIR: a seeded sample of the last timed step's outputs, DIR/<name>.npy.
 
 --impl reference times the reference's own CPU implementation of the path on the
 host cores: oracle/_ref (the reference's headers compiled against the Eigen-API
@@ -60,7 +51,8 @@ D = 128
 M = 10
 SEED = 12345
 LOG2_B = 20
-HBM_FALLBACK_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_FALLBACK_GBS = 3350.0  # NVIDIA H100 SXM data sheet (HBM3), used when MEASURED_PEAKS.json is absent
+DUMP_INSTANCES = 16384    # --dump-outputs: instances sampled from the batch (about 33 MB of float64 at d = 128)
 METRIC = "batched L-BFGS instances/sec (Rosenbrock d=128)"
 
 
@@ -198,16 +190,23 @@ def run_reference(args):
     return 0
 
 
-def load_instr_mix():
-    """FP64-pipe / DMMA warp instructions per solver iteration of the headline kernel, from the ncu
-    source-level counts committed under profiles/ (tools/ncu_summary.py writes the file)."""
-    for name in ("r02_instr_mix.json", "r01_instr_mix.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            j = json.load(open(p))
-            j["source"] = f"profiles/{name}"
-            return j
-    return None
+def dump_outputs(out_dir, state, prog):
+    """The last timed step's outputs for a fixed, seeded sample of the instances (sample_index.npy), as float64."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    B = state.x.shape[0]
+    idx = np.sort(np.random.default_rng(SEED).choice(B, size=min(B, DUMP_INSTANCES), replace=False))
+    sel = torch.from_numpy(idx).to(state.x.device)
+    arrays = {"sample_index": idx, "x": state.x, "value": state.value, "gradient": state.gradient,
+              "num_iterations": prog.num_iterations, "status": prog.status, "nfev": prog.nfev,
+              "x_delta": prog.x_delta, "f_delta": prog.f_delta, "gradient_norm": prog.gradient_norm}
+    for name, a in arrays.items():
+        if a is None:
+            continue
+        if isinstance(a, torch.Tensor):
+            a = a[sel].cpu().numpy()
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def parity_sample(x0, state, prog, n_samples: int, threads: int):
@@ -236,9 +235,9 @@ def parity_sample(x0, state, prog, n_samples: int, threads: int):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=3, help="timed steps (at least 1)")
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])  # b200: this project's kernels
     ap.add_argument("--log2-batch", type=int, default=LOG2_B, help="per-GPU batch = 2^this")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
     ap.add_argument("--ref-seconds", type=float, default=6.0,
@@ -246,7 +245,11 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the strong-scaling and other-config records")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (a seeded sample of the instances) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
 
     if args.impl == "reference":
         return run_reference(args)
@@ -320,6 +323,8 @@ def main():
     all_done = bool((bitmap == -1).all().item())  # every bit set
     value = world * B * args.steps / (ms * 1e-3)
     clk = clocks.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, state, prog)
 
     # kernel-only timing for the roofline (CUDA events inside cno_minimize, same stream)
     kms = []
@@ -336,38 +341,8 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+        peak, peak_src = HBM_FALLBACK_GBS, "H100 SXM data sheet (not measured)"
     achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
-    traffic = None
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tpath):
-            tj = json.load(open(tpath))
-            if tj.get("batch") == B:
-                traffic = tj["dram_bytes_read"] + tj["dram_bytes_write"]
-            break
-
-    # the resource that binds: the FP64 datapath (vector FP64 pipe + FP64 tensor-core MMA)
-    compute = None
-    mix = load_instr_mix()
-    if mix is not None:
-        props = torch.cuda.get_device_properties(dev)
-        sm_clock_hz = (clk["sm_mhz"] or clk["sm_max_mhz"] or 1965.0) * 1e6
-        total_iters = float(iters.astype(np.int64).sum())
-        # one FP64 warp instruction occupies a sub-partition's 16-lane FP64 pipe for 2 cycles; a DMMA.8x8x4
-        # for `dmma_cycles` (measured: tools/fp64_pipe_probe.cu) -- expressed in FP64-instruction equivalents
-        dmma_equiv = mix.get("dmma_cycles", 16.0) / 2.0
-        per_iter = mix["fp64_per_iteration"] + dmma_equiv * mix["dmma_per_iteration"]
-        ach = per_iter * total_iters / (kernel_ms * 1e-3)
-        pk = props.multi_processor_count * 4 * 0.5 * sm_clock_hz
-        compute = {"bound": "fp64", "achieved": ach / 1e9, "peak": pk / 1e9, "unit": "G FP64 warp-instr/s",
-                   "frac": ach / pk, "fp64_per_iteration": mix["fp64_per_iteration"],
-                   "dmma_per_iteration": mix["dmma_per_iteration"], "dmma_fp64_equivalents": dmma_equiv,
-                   "instr_per_iteration": mix.get("instr_per_iteration"),
-                   "sm_clock_mhz": sm_clock_hz / 1e6, "instr_mix_source": mix["source"],
-                   "note": "FP64-pipe warp instructions + FP64 tensor-core MMAs (at their measured pipe "
-                           "occupancy) per solver iteration x this run's iterations / kernel time, against "
-                           "SMs x 4 x 0.5 warp-instr/clk x the SM clock sampled during the run"}
 
     # ---- parity: strided instances of the timed batch against the CPU oracle ----
     parity = parity_sample(x0, state, prog, 256, threads) if rank == 0 else None
@@ -431,7 +406,7 @@ def main():
                 "workload": "Rosenbrock d=128 fp64, L-BFGS m=10, default stopping preset "
                             "(BASELINE.json configs[1])",
                 "batch_per_gpu": B, "global_batch": world * B, "parallelism": f"shard{world}",
-                "l2": "x0 is 1 GiB per GPU (> 126 MB L2); no flush needed",
+                "l2": "x0 is 1 GiB per GPU (> 50 MB L2); no flush needed",
                 "start_generator": f"splitmix64 counter stream, seed {SEED}, U(-2,2)",
                 "timed_region": "Minimize kernel + done-bitmap kernel + bitmap all-gather + D2H of status",
                 "mean_iterations": float(iters.mean()), "mean_nfev": float(nfev.mean()),
@@ -443,15 +418,12 @@ def main():
             "gpu_launches": args.steps * 2,  # lbfgs_minimize_kernel + done_bitmap_kernel per step
             "roofline": {
                 "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic,
+                "frac": achieved / peak,
                 "peak_source": peak_src, "kernel": "lbfgs_minimize_kernel<RosenbrockFn<double,128>,10>",
                 "kernel_ms": kernel_ms, "algorithmic_bytes_per_launch": alg_bytes,
-                "compute": compute,
                 "note": "hbm: algorithmic bytes = state-streaming model w*d*(2k+6)/iteration; the fused "
-                        "kernel keeps the (s,y) history on chip (shared memory + Tensor Memory), so this "
-                        "frac > 1 means the traffic was removed, not that work was skipped (see `parity`); "
-                        "`traffic` = ncu DRAM bytes per launch.  The resource that BINDS the kernel is the "
-                        "FP64 datapath: `compute` is the fraction to read.",
+                        "kernel keeps the (s,y) history on chip (shared memory), so this "
+                        "frac > 1 means the traffic was removed, not that work was skipped (see `parity`).",
             },
             "parity": parity,
             "cpu_baseline": cpu,

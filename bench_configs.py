@@ -21,7 +21,7 @@ DEV = "cuda"
 
 def peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    return float(json.load(open(p))["hbm_gbs"]) if os.path.exists(p) else 6650.0
+    return float(json.load(open(p))["hbm_gbs"]) if os.path.exists(p) else 3350.0  # H100 SXM data sheet
 
 
 def run(name, solver, fn, x0, bytes_fn, reps=3, extra=None):
@@ -42,17 +42,7 @@ def run(name, solver, fn, x0, bytes_fn, reps=3, extra=None):
            "grid": pr.launch.grid, "warps_per_cta": pr.launch.warps_per_cta,
            "dynamic_smem": pr.launch.dynamic_smem}
     out.update(extra or {})
-    bind = binding_pipes().get(name.split()[0])
-    if bind:
-        out["binding"] = bind
     return out
-
-
-def binding_pipes():
-    """Per-config summary of the ncu capture (which pipe binds the kernel), written by hand from
-    profiles/r02_*_ncu_full.txt into profiles/r02_binding.json."""
-    p = os.path.join(ROOT, "profiles", "r02_binding.json")
-    return json.load(open(p)) if os.path.exists(p) else {}
 
 
 def lbfgs_bytes(w, d, m=10):

@@ -1,8 +1,8 @@
-"""cppnumericalsolvers_b200 -- B200-native batched unconstrained minimisation.
+"""cppnumericalsolvers_b200 -- H100-native batched unconstrained minimisation.
 
 Host-side mirror of cppoptlib's solver::{Lbfgs,Lbfgsb,Bfgs,NewtonDescent,GradientDescent,
 ConjugatedGradientDescent}::Minimize
-with a batch axis; the compute is hand-written sm_100a CUDA in libcno.so behind
+with a batch axis; the compute is hand-written sm_90a CUDA in libcno.so behind
 the C ABI of include/cno.h.  No CPU fallback.
 """
 from . import _lib  # noqa: F401

@@ -1,7 +1,6 @@
-"""Builds libcno.so (hand-written sm_100a CUDA + the extern "C" layer) in-tree.
+"""Builds libcno.so (hand-written sm_90a CUDA + the extern "C" layer) in-tree.
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the
-GPU box with the gpurun snapshot.  -fmad=false is part of the arithmetic
+nvcc cross-compiles without a GPU; the .so is a build product (git-ignored).  -fmad=false is part of the arithmetic
 specification (no FMA contraction, like the reference's canonical build).
 """
 from __future__ import annotations
@@ -15,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcno.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",
     "-shared", "-Xcompiler", "-fPIC",
@@ -49,7 +48,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
 def build_cpp_tests(verbose: bool = False) -> list:
     """Compiles the C++ host-API programs under tests/cpp (g++ and nvcc translation
-    units) into tests/cpp/build/ (git-ignored, travels to the GPU box)."""
+    units) into tests/cpp/build/ (git-ignored)."""
     root = os.path.dirname(HERE)
     src = os.path.join(root, "tests", "cpp")
     out = os.path.join(src, "build")
@@ -73,7 +72,7 @@ def build_cpp_tests(verbose: bool = False) -> list:
     exes.append(os.path.join(out, "sharded_nccl"))
     nvcc = os.environ.get("NVCC", f"{cuda}/bin/nvcc")
     xlink = ["-Xlinker", f"-rpath={HERE}"]
-    dev_flags = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    dev_flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
                  "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false"]
     jobs = [(os.path.join(src, "user_functor.cu"), os.path.join(out, "user_functor"), []),
             # user functors + composites as a shared library for the Python parity tests (tests/usertest_binding.py)

@@ -4,7 +4,7 @@ AugmentedLagrangianConfig / AugmentedLagrangeState / AugmentedLagrangian) over t
 include/cno_al.h.
 
 The algorithm is pinned on the CPU (oracle/cno_al_oracle.h, tests/test_al_oracle.py); the device path
-equals it bit for bit on a B200 (tests/test_al_gpu.py)."""
+equals it bit for bit on the GPU (tests/test_al_gpu.py)."""
 from __future__ import annotations
 
 import ctypes as C

@@ -2,7 +2,7 @@
 // table of kernels instantiated for the built-in objective families.
 //
 // Build (see cppnumericalsolvers_b200/build.py):
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false ...
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false ...
 // -fmad=false is part of the arithmetic specification: the reference's
 // canonical build forms no FMAs (generator.bzl:13, Dockerfile.test:111).
 #include <cuda_runtime.h>
@@ -235,12 +235,11 @@ int newton_dense_quadratic(const LaunchArgs& a) {
       cno::DenseQuadraticFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
 }
 // CNO_POLICY_DMMA_LU: d = 64 fp64 dense quadratic, blocked LU with the trailing update on the FP64 tensor core
-// (csrc/cno_newton_dmma.cuh).  kLayout = the CTA's warp population (matrices in shared memory / Tensor Memory / both).
-template <int kLayout>
+// (csrc/cno_newton_dmma.cuh).
 int launch_newton_dmma(const cno::DenseQuadraticDmmaFn& fn, const LaunchArgs& a) {
   using Fn = cno::DenseQuadraticDmmaFn;
-  using SM = cno::NewtonDmmaSmem<kLayout>;
-  auto kernel = cno::newton_dmma_minimize_kernel<Fn, kLayout>;
+  using SM = cno::NewtonDmmaSmem;
+  auto kernel = cno::newton_dmma_minimize_kernel<Fn>;
   const size_t smem = SM::kBytes;
   CNO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int sms = 0;
@@ -271,14 +270,7 @@ int newton_dense_quadratic_dmma(const LaunchArgs& a) {
   cno::DenseQuadraticDmmaFn fn;
   fn.data = static_cast<const double*>(p->data);
   fn.stride = (long long)p->data_stride;
-  // CNO_NEWTON_DMMA_LAYOUT = 0 / 1 / 2 picks the warp population (measurement knob; results are identical)
-  const char* env = getenv("CNO_NEWTON_DMMA_LAYOUT");
-  const int layout = env ? atoi(env) : 3;
-  if (layout == 0) return launch_newton_dmma<0>(fn, a);
-  if (layout == 1) return launch_newton_dmma<1>(fn, a);
-  if (layout == 2) return launch_newton_dmma<2>(fn, a);
-  if (layout == 4) return launch_newton_dmma<4>(fn, a);
-  return launch_newton_dmma<3>(fn, a);
+  return launch_newton_dmma(fn, a);
 }
 template <class T, int D>
 int newton_rosenbrock(const LaunchArgs& a) {
@@ -1294,8 +1286,11 @@ int cno_fill_uniform(int dtype, void* dst, int64_t first, int64_t count, uint64_
   if (count == 0) return CNO_OK;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int block = 256;
+  int sms = 0;
+  const int rc = device_sm_count(&sms);
+  if (rc) return rc;
   long long blocks = (count + block - 1) / block;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;  // grid-stride loop: 16 blocks per SM
   if (dtype == CNO_F64)
     fill_uniform_kernel<double><<<(int)blocks, block, 0, s>>>((double*)dst, first, count, seed, lo, hi);
   else

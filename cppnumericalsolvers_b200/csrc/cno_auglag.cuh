@@ -1,8 +1,8 @@
 // cno_auglag.cuh -- batched AugmentedLagrangian<Problem, Lbfgs>::Minimize: the
 // composite device functor the fused L-BFGS kernel minimises, and the kernels of the
-// outer loop (one warp per instance, sm_100a).
+// outer loop (one warp per instance, sm_90a).
 //
-// Parity: bit-identical on a B200 to the pinned CPU oracle (oracle/cno_oracle_impl.inc:
+// Parity: bit-identical on the GPU to the pinned CPU oracle (oracle/cno_oracle_impl.inc:
 // eval_auglag, al_minimize_one) and to the reference-headers fixtures tests/golden/al_*.npz
 // (tests/test_al_gpu.py).  DESIGN.md 8.
 //

@@ -1,5 +1,5 @@
 // cno_bfgs.cuh -- batched Bfgs<F>::Minimize (dense inverse Hessian), one warp
-// per instance, whole Solver::Minimize loop in one persistent kernel (sm_100a).
+// per instance, whole Solver::Minimize loop in one persistent kernel (sm_90a).
 //
 // Reference path (include/cppoptlib/...):
 //   solver/solver.h:181-224   Solver::Minimize driver loop
@@ -8,7 +8,7 @@
 //                             MoreThuente::Search, rank-2 update (N&W 6.17)
 //   solver/progress.h:153-327 Progress::Update
 //
-// B200 design (D <= 32): lane i keeps ROW i of the inverse Hessian in registers
+// Design (D <= 32): lane i keeps ROW i of the inverse Hessian in registers
 // (D doubles; the update keeps H bitwise symmetric, so row i == column i) for
 // the instance's whole lifetime -- H never touches HBM, and not even shared
 // memory.  Vectors (x, g, d, s, y, Hy) are one element per lane.  The two GEMVs

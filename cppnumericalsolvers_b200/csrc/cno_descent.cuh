@@ -1,6 +1,6 @@
 // cno_descent.cuh -- batched GradientDescent<F>::Minimize and
 // ConjugatedGradientDescent<F>::Minimize, one warp per instance, the whole
-// Solver::Minimize loop in one persistent kernel (sm_100a).
+// Solver::Minimize loop in one persistent kernel (sm_90a).
 //
 // Reference path (include/cppoptlib/...):
 //   solver/solver.h:181-224                      Solver::Minimize driver loop

@@ -18,7 +18,7 @@ evaluate_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x, const lo
   using T = typename Fn::Scalar;
   constexpr int D = Fn::Dim;
   constexpr int E = Shape<D>::E;
-  static_assert(StageElems<Fn>::value == 0 && FnTmemCols<Fn>::value == 0,
+  static_assert(StageElems<Fn>::value == 0,
                 "evaluate_kernel: functors that stage per-instance data are evaluated by their solver kernels only");
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * kEvalWarps;

@@ -16,7 +16,6 @@
 //
 // Optional members the solver kernels look for (traits in cno_device.cuh):
 //   kStageElems + init_stage()/stage()  per-instance data staged into the warp's shared-memory slice (StageElems)
-//   kTmemCols                           a Tensor Memory window per instance (FnTmemCols)
 //   kPreferredWarps                     resident warps per CTA the functor's register budget allows (FnPreferredWarps)
 //   active(instance)                    instances the kernel skips (FnSkipsInstances; AugLagFn)
 //   kHelperWarps = 1 + helper()/release_helper()   a second warp per instance that the functor drives through a
@@ -43,7 +42,9 @@ struct RosenbrockFn {
   static constexpr int E = Shape<D>::E;
 
   static constexpr bool kHasPartial = true;
-  // fp64, 4 elements per lane, default policy: light enough for 20 resident warps (cno_device.cuh: FnPreferredWarps)
+  // fp64, 4 elements per lane, default policy: the register budget allows 20 resident warps (cno_device.cuh:
+  // FnPreferredWarps).  Shared memory decides where the history is larger: at m = 10 (20 KiB per instance) 11 warps fit,
+  // at m = 5 the full 20.
   static constexpr int kPreferredWarps = (sizeof(T) == 8 && E == 4 && std::is_same<P, PolicyFast>::value) ? 20 : 16;
   __device__ __forceinline__ T operator()(const EvalCtx& c, const T (&x)[E],
                                           T (*grad)[E]) const {
@@ -179,7 +180,7 @@ struct HalfSquaredNormFn {
 // no matrix on chip (Lbfgs, and AugmentedLagrangian's batched "QP with affine constraints" use).
 // Reference analogue: src/examples/debug.cc:43-65; src/test/augmented_lagrangian_test.cc:78-176
 // (QuadraticAt12 / QuadraticAt20).  (Ax)_i = sum_j A_ij x_j, j ascending from the first product;
-// x_j is broadcast from its owner lane.  Parity: tests/test_al_gpu.py (B200) and the CPU warp emulation
+// x_j is broadcast from its owner lane.  Parity: tests/test_al_gpu.py (GPU) and the CPU warp emulation
 // (tests/test_device_emulated.py), both bit for bit against the oracle.
 template <class T, int D>
 struct DenseQuadraticGlobalFn {

@@ -1,5 +1,5 @@
 // cno_lbfgs.cuh -- batched Lbfgs<F, m>::Minimize, one warp per instance, the
-// whole Solver::Minimize loop fused into ONE persistent kernel (sm_100a).
+// whole Solver::Minimize loop fused into ONE persistent kernel (sm_90a).
 //
 // Reference path (include/cppoptlib/...):
 //   solver/solver.h:181-224   Solver::Minimize driver loop
@@ -9,13 +9,12 @@
 //   linesearch/more_thuente.h MoreThuente::Search / cvsrch / cstep
 //   solver/progress.h:153-327 Progress::Update
 //
-// B200 design: grid = #SMs persistent CTAs; each warp pulls instance ids from
+// Design: grid = #SMs persistent CTAs; each warp pulls instance ids from
 // a global atomic queue (instances run 20..10000 iterations, so retire +
 // refill is what keeps all warps busy through the tail).  The m-deep (s, y)
 // history of the instance a warp is working on stays ON CHIP for the instance's
-// whole lifetime: s_i in the warp's private slice of shared memory and -- when a
-// lane's slice is 4 doubles (d = 128 fp64) -- y_i in Tensor Memory (YHist), which
-// lifts the shared-memory cap on resident warps (11 -> 16 per SM); x, g, the
+// whole lifetime, in the warp's private slice of shared memory (at d = 128 fp64
+// that is 20 KB per instance: 11 resident warps per SM); x, g, the
 // search direction and the trial point live in registers.  HBM is touched twice
 // per instance: one coalesced vectorised read of x0 and one write of the result.
 // Inner products: in-lane tree, then the cross-lane sum on the FP64 tensor core
@@ -32,40 +31,29 @@
 
 namespace cno {
 
-template <class T, int D, int M, int kStage = 0, int kScratchPerLane = 0, int kFnTmem = 0, int kMaxW = 16, int kHelpers = 0>
+template <class T, int D, int M, int kStage = 0, int kScratchPerLane = 0, int kMaxW = 16, int kHelpers = 0>
 struct LbfgsSmem {
   static constexpr int E = Shape<D>::E;
   static constexpr int kVec = 32 * E;                        // elements per stored vector
   static constexpr int kScalars = 2 * M + CNO_MAX_PAST + 32 * kScratchPerLane;  // rho[M], alpha[M], f ring, policy scratch
-  // y-history in Tensor Memory (8 columns per stored vector, M*8 <= 128 columns per
-  // warp at 16 warps/CTA) when a lane's slice is exactly 4 doubles: this lifts the
-  // shared-memory cap on resident warps (11 -> 16 per SM at d = 128 fp64).
-  static constexpr bool kTmemY = (sizeof(T) == 8 && E == 4 && M * 8 <= 128 && kStage == 0);
-  static constexpr int kHistElems = (kTmemY ? 1 : 2) * M * kVec + ((kScalars + 3) / 4) * 4;  // S (, Y) + scalars
+  static constexpr int kHistElems = 2 * M * kVec + ((kScalars + 3) / 4) * 4;  // S, Y + scalars
   static constexpr int kWarpElems = kHistElems + kStage;     // + the functor's staged block
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
   // warps per CTA: as many as fit in 227 KB, at most 16 (register budget).
   static constexpr int kMaxSmem = 227 * 1024;
   static constexpr int kWarpsFit = (int)(kMaxSmem / kWarpBytes);
-  // a functor that keeps data in Tensor Memory limits the warps per lane quadrant
   static constexpr int kMaxWarps = kMaxW;  // register budget: 65536 / (32 * warps) per thread (FnPreferredWarps)
-  static constexpr int kTmemColsPerWarp = M * 8;             // a stored y vector = 8 columns of the warp's 32 lanes
-  static constexpr int kTmemYCap = kTmemY ? 4 * (512 / kTmemColsPerWarp) : kMaxWarps;  // warps per lane quadrant x 4
-  static constexpr int kTmemWarpCap = kFnTmem > 0 ? 4 * (512 / kFnTmem) : kTmemYCap;
-  static constexpr int kCap = kTmemWarpCap < kMaxWarps ? kTmemWarpCap : kMaxWarps;
-  static constexpr int kWarps = kWarpsFit > kCap ? kCap : (kWarpsFit < 1 ? 1 : kWarpsFit);
+  static constexpr int kWarps = kWarpsFit > kMaxWarps ? kMaxWarps : (kWarpsFit < 1 ? 1 : kWarpsFit);
   // Functors with a helper warp per instance (FnHelperWarps): solver warps 0 .. kWarps-1, the helper of solver warp t is
-  // warp kHelperBase + t (with 5 solver warps: another sub-partition than its solver warp, 2-3 warps per sub-partition);
-  // the functor's Tensor Memory window belongs to the HELPER (its own lane quadrant).
+  // warp kHelperBase + t.
   static constexpr int kHelperBase = kWarps;
   static constexpr int kThreads = 32 * (kHelpers > 0 ? 2 * kWarps : kWarps);
 };
 
-// y-history accessors: shared memory (chunk-interleaved) or Tensor Memory.
-template <class T, int E, bool kTmem>
-struct YHist;
+// y-history accessor: the warp's shared-memory slice (chunk-interleaved).  A load is issued before the reduction it
+// overlaps and consumed after it (issue / wait).
 template <class T, int E>
-struct YHist<T, E, false> {
+struct YHist {
   T* base;
   int lane;
   struct Pending {};
@@ -73,15 +61,6 @@ struct YHist<T, E, false> {
   __device__ __forceinline__ void issue(int slot, T (&v)[E], Pending&) const { SmemVec<T, E>::load(base + slot * 32 * E, lane, v); }
   __device__ __forceinline__ void wait(T (&)[E], Pending&) const {}
   __device__ __forceinline__ void fence_store() const {}
-};
-template <>
-struct YHist<double, 4, true> {
-  uint32_t taddr;  // this warp's TMEM window
-  struct Pending { uint32_t r[8]; };
-  __device__ __forceinline__ void store(int slot, const double (&v)[4]) const { tmem_st4(taddr + slot * 8, v); }
-  __device__ __forceinline__ void issue(int slot, double (&)[4], Pending& p) const { tmem_ld4_issue(taddr + slot * 8, p.r); }
-  __device__ __forceinline__ void wait(double (&v)[4], Pending& p) const { tmem_ld4_wait(p.r, v); }
-  __device__ __forceinline__ void fence_store() const { tmem_wait_st(); }
 };
 
 // progress.h:153-327 on warp-uniform scalars (FunctionState branch).  The
@@ -192,7 +171,7 @@ template <class Fn, int M, bool kResume = false, class LS = LsMoreThuente>
 struct LbfgsPlan {
   static constexpr bool kPlain = std::is_same<LS, LsMoreThuente>::value && !IsSecondMode<Fn>::value && !kResume;
   using SM = LbfgsSmem<typename Fn::Scalar, Fn::Dim, M, StageElems<Fn>::value,
-                       PolicyScratch<typename PolicyOf<Fn>::type>::kElemsPerLane, FnTmemCols<Fn>::value,
+                       PolicyScratch<typename PolicyOf<Fn>::type>::kElemsPerLane,
                        kPlain ? FnPreferredWarps<Fn>::value : 16, FnHelperWarps<Fn>::value>;
 };
 
@@ -208,7 +187,6 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   constexpr int kStage = StageElems<Fn>::value;
   using P = typename PolicyOf<Fn>::type;
   constexpr bool kSecond = IsSecondMode<Fn>::value;  // lbfgs.h:116-118 has_diagonal_preconditioner
-  constexpr int kFnTmem = FnTmemCols<Fn>::value;
   using SM = typename LbfgsPlan<Fn, M, kResume, LS>::SM;
   using SV = SmemVec<T, E>;
   constexpr T eps = Num<T>::eps;
@@ -220,36 +198,9 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   // the instance slot this warp works for: its own, or (helper warps) the one of its solver warp
   const int slot = (kHelpers > 0 && warp >= SM::kHelperBase) ? warp - SM::kHelperBase : warp;
   T* const S = reinterpret_cast<T*>(smem_raw) + (size_t)slot * SM::kWarpElems;
-  T* const Ysm = S + M * SM::kVec;     // (unused when the y-history lives in TMEM)
-  T* const rho_s = S + (SM::kTmemY ? 1 : 2) * M * SM::kVec;  // 1 / (s_i . y_i) per slot
-  uint32_t tmem_base = 0;
-  constexpr bool kAllocTmem = SM::kTmemY || (kFnTmem > 0);
-  static_assert(!(SM::kTmemY && kFnTmem > 0), "one Tensor Memory user per kernel");
-  if constexpr (kAllocTmem) {
-#ifdef CNO_WARP_EMULATION  // tests/emu: the emulated warp's Tensor Memory window starts at column 0
-    tmem_base = 0;
-#else
-    __shared__ uint32_t tmem_base_s;
-    if (warp == 0) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                       (uint32_t)__cvta_generic_to_shared(&tmem_base_s)),
-                   "n"(512));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    tmem_base = tmem_base_s;
-#endif
-  }
-  YHist<T, E, SM::kTmemY> Y;
-  if constexpr (SM::kTmemY) {
-    Y.taddr = tmem_base + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((slot >> 2) * SM::kTmemColsPerWarp);
-  } else {
-    Y.base = Ysm;
-    Y.lane = lane;
-  }
-  typename YHist<T, E, SM::kTmemY>::Pending ypend;
+  T* const rho_s = S + 2 * M * SM::kVec;  // 1 / (s_i . y_i) per slot
+  const YHist<T, E> Y{S + M * SM::kVec, lane};
+  typename YHist<T, E>::Pending ypend;
   T* const alpha = rho_s + M;
   T* const ring = alpha + M;
   // policy scratch (PolicyEigenSSE2): 16-byte aligned tail of the scalar block; handed to
@@ -258,18 +209,13 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   const RedCtx<T> rc{red_scratch, lane};
   void* const stage_ptr = (kStage > 0) ? static_cast<void*>(S + SM::kHistElems) : static_cast<void*>(red_scratch);
   uint32_t stage_parity = 0;
-  // (with helper warps the window is the helper's: its own lane quadrant, one window per helper of that quadrant)
-  const uint32_t fn_tmem = (kFnTmem > 0)
-                               ? tmem_base + ((uint32_t)(32 * (warp & 3)) << 16) +
-                                     (uint32_t)(((kHelpers > 0 ? (warp >= SM::kHelperBase ? warp - SM::kHelperBase : 0) : warp) >> 2) * kFnTmem)
-                               : 0u;
   bool solver_warp = true;
   if constexpr (kHelpers > 0) {
     solver_warp = uni(warp < SM::kWarps);
-    if (uni(warp >= SM::kHelperBase)) fn.helper(EvalCtx{lane, 0, stage_ptr, fn_tmem, slot});  // until its solver warp releases it
+    if (uni(warp >= SM::kHelperBase)) fn.helper(EvalCtx{lane, 0, stage_ptr, slot});  // until its solver warp releases it
   }
   if constexpr (kStage > 0) {
-    if (solver_warp) fn.init_stage(EvalCtx{lane, 0, stage_ptr, fn_tmem, slot});
+    if (solver_warp) fn.init_stage(EvalCtx{lane, 0, stage_ptr, slot});
   }
 
   for (; solver_warp;) {
@@ -281,7 +227,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     if constexpr (FnSkipsInstances<Fn>::value) {  // e.g. AugLagFn: the instance's outer loop has finished
       if (uni(!fn.active((long long)b))) continue;
     }
-    const EvalCtx ctx{lane, (long long)b, stage_ptr, fn_tmem, slot};
+    const EvalCtx ctx{lane, (long long)b, stage_ptr, slot};
     if constexpr (kStage > 0) fn.stage(ctx, stage_parity);  // per-instance data -> shared memory (TMA)
 
     T x[E], g[E];
@@ -637,15 +583,8 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     __syncwarp();
   }
   if constexpr (kHelpers > 0) {
-    if (solver_warp) fn.release_helper(EvalCtx{lane, 0, stage_ptr, fn_tmem, slot});
+    if (solver_warp) fn.release_helper(EvalCtx{lane, 0, stage_ptr, slot});
   }
-#ifndef CNO_WARP_EMULATION
-  if constexpr (kAllocTmem) {
-    __syncthreads();  // every warp is done with its TMEM window
-    if (warp == 0)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-  }
-#endif
 }
 
 }  // namespace cno

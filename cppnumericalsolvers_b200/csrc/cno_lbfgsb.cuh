@@ -1,5 +1,5 @@
 // cno_lbfgsb.cuh -- batched Lbfgsb<F, m = 5>::Minimize (box constraints l <= x <= u), one warp per instance, the
-// whole overridden Minimize loop in one persistent kernel (sm_100a).
+// whole overridden Minimize loop in one persistent kernel (sm_90a).
 //
 // Reference path (include/cppoptlib/solver/lbfgsb.h):
 //   :78-81    Lbfgsb() preset (default + f_delta = 2.22e-9 relative)      -> cno_lbfgsb_default_stop
@@ -11,7 +11,7 @@
 //   :238-286  the overridden Minimize loop: projected-gradient stop test on top of Progress::Update
 //   :322-446  GetGeneralizedCauchyPoint      :451-475 FindAlpha      :477-525 SubspaceMinimization
 //
-// B200 design.  x, g, the Cauchy point and the search direction live in registers (E = ceil(d/32) elements per
+// Design.  x, g, the Cauchy point and the search direction live in registers (E = ceil(d/32) elements per
 // lane); the m-deep (y, s) history (2 x 5 x d) and a compaction buffer live in the warp's shared-memory slice;
 // the 2k-vectors of the compact representation (p, c, w_b, v: 2k <= 10 entries) are ONE register per lane (entry i
 // in lane i), so their inner products are ordinary warp sums and the (2k x 2k) solves with the LU factors of MM

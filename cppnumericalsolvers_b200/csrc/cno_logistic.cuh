@@ -7,13 +7,10 @@
 // The block is read twice per evaluation (margins, gradient) and an instance
 // needs ~40 evaluations, so it is staged ONCE per instance and stays ON CHIP:
 // HBM traffic = one read of the block per instance instead of one per
-// evaluation.  The block is split over both on-chip stores so more instances are
-// resident per SM (5 instead of 3), and over TWO WARPS per instance: the samples
-// come in two chunks of 128; chunk 0 of every feature and y go to the instance's
-// shared-memory slice by TMA bulk copies (cp.async.bulk + mbarrier) and belong to
-// the solver warp, chunk 1 of every feature goes to the Tensor Memory window of the
-// instance's helper warp (coalesced loads + tcgen05.st; 4 columns per feature), a
-// warp of another sub-partition.
+// evaluation.  The block arrives in the instance's shared-memory slice by one TMA
+// bulk copy (cp.async.bulk + mbarrier), in its global layout, and is evaluated by
+// TWO WARPS per instance: the samples come in two chunks of 128; chunk 0 of every
+// feature belongs to the solver warp, chunk 1 to the instance's helper warp.
 //
 // Lane ownership inside the functor: lane l owns samples 128c + 4l .. 4l+3 of
 // its warp's chunk c, so every shared-memory access is a contiguous
@@ -26,8 +23,7 @@
 #include "cno_device.cuh"
 #include "cno_newton.cuh"  // TMA + mbarrier helpers
 
-// Loop-size knobs of the functor (measured on B200, BASELINE config 3, kernel ms for B = 2^18 -- round features /
-// margin batch: 8/8 111.9, 16/8 105.5, 8/16 110.2, 16/16 110.2, 8/4 113.0, 4/8 128.2)
+// Loop-size knobs of the functor: features per gradient round / per batch of margin loads
 #ifndef CNO_LOGISTIC_ROUND_FEATURES
 #define CNO_LOGISTIC_ROUND_FEATURES 16
 #endif
@@ -102,13 +98,10 @@ struct LogisticFn {
   static_assert(N == 256, "two chunks of 128 samples (32 lanes x 4): one per warp of the team");
   static_assert(D % 16 == 0, "the gradient is built in rounds of kRF features");
   static constexpr int kBlockElems = D * N + N;  // [Xt | y] in global memory
-  static constexpr int kTmemCols = D * 4;        // the helper warp's window: chunk 1, 4 columns per feature
   static constexpr int kWvec = ((D + 3) / 4) * 4;
   // Features per gradient round (each warp owns kG = kRF / 2 of them: its butterflies in flight).  Code size matters
-  // here: two or three warps share a sub-partition's 6 KB instruction cache (L0).  With the four samples' losses
-  // unrolled (5.5 KB of straight-line code per warp and evaluation) every issued instruction cost one instruction-fetch
-  // stall (ncu: stall_no_inst = stall_selected = 15 % of the samples); rolled (losses()), fetch stalls are 2 % and the
-  // loop sizes below are the measured optimum.
+  // here: the solver and helper warps of several instances share a sub-partition's instruction cache (L0), so the four
+  // samples' losses are a rolled loop (losses()) rather than straight-line code.
   static constexpr int kRF = CNO_LOGISTIC_ROUND_FEATURES;
   static constexpr int kG = kRF / 2;
   // A helper warp per instance (FnHelperWarps).  The split keeps every sum of the arithmetic definition in its order:
@@ -121,10 +114,10 @@ struct LogisticFn {
   //    its lane partials.
   static constexpr int kHelperWarps = 1;
   static constexpr int kRounds = D / kRF;
-  // shared-memory slice of the team (elements): chunk 0 of every feature | y | broadcast copy of w | mbarrier (8 bytes) |
-  // exchange area: partials for the solver warp [2 buffers][8][32], for the helper [2][8][32], the helper's loss
-  // partials [32], its gradient sums [D/2], the command word + instance index
-  static constexpr int kX0 = 0, kY = D * 128, kW = kY + N, kBar = kW + kWvec;
+  // shared-memory slice of the team (elements): Xt (feature i: chunk 0 | chunk 1) | y | broadcast copy of w |
+  // mbarrier (8 bytes) | exchange area: partials for the solver warp [2 buffers][8][32], for the helper [2][8][32], the
+  // helper's loss partials [32], its gradient sums [D/2], the command word
+  static constexpr int kX = 0, kY = D * N, kW = kY + N, kBar = kW + kWvec;
   static constexpr int kXchgOff = ((kBar + 8 / (int)sizeof(T) + 3) / 4) * 4;
   static constexpr int kToL = 0, kToH = 2 * 8 * 32, kXLoss = 2 * kToH, kXGrad = kXLoss + 32, kXCmd = kXGrad + D / 2,
                        kXchgElems = kXCmd + 4;
@@ -141,29 +134,21 @@ struct LogisticFn {
     return reinterpret_cast<volatile int*>(xchg(c) + kXCmd);
   }
 
-  // once per instance: chunk 0 of every feature + y -> shared memory (TMA bulk copies issued by the solver warp's
-  // lanes), chunk 1 -> the helper's Tensor Memory window (the helper's own loads and stores)
+  // once per instance: the block [Xt | y] -> shared memory, one TMA bulk copy issued by the solver warp; both warps of
+  // the team wait for it on the mbarrier (the helper when it picks up kCmdStage)
   __device__ __forceinline__ void stage(const EvalCtx& c, uint32_t& parity) const {
     T* blk = static_cast<T*>(c.stage);
     uint64_t* bar = reinterpret_cast<uint64_t*>(blk + kBar);
-    const T* src = data + c.instance * stride;
     __syncwarp();
+    fence_proxy_async();  // the previous instance's reads of the slice come before the copy overwrites it
     if (c.lane == 0) {
-      volatile int* cw = cmd_word(c);
-      cw[0] = kCmdStage;
-      cw[1] = (int)(uint32_t)(unsigned long long)c.instance;
-      cw[2] = (int)(uint32_t)((unsigned long long)c.instance >> 32);
-      fence_proxy_async();
-      mbar_expect_tx(bar, (uint32_t)((D * 128 + N) * sizeof(T)));
-      tma_bulk_g2s(blk + kY, src + D * N, (uint32_t)(N * sizeof(T)), bar);
+      cmd_word(c)[0] = kCmdStage;
+      mbar_expect_tx(bar, (uint32_t)(kBlockElems * sizeof(T)));
+      tma_bulk_g2s(blk + kX, data + c.instance * stride, (uint32_t)(kBlockElems * sizeof(T)), bar);
     }
     team_sync(c.team);  // the helper picks the command up (and every lane is past the expect_tx)
-    fence_proxy_async();
-    for (int i = c.lane; i < D; i += 32)
-      tma_bulk_g2s(blk + kX0 + i * 128, src + i * N, (uint32_t)(128 * sizeof(T)), bar);
     mbar_wait(bar, parity);
     parity ^= 1u;
-    team_sync(c.team);  // y is in shared memory for the helper too; its Tensor Memory stores are complete
   }
   __device__ __forceinline__ void init_stage(const EvalCtx& c) const {
     T* blk = static_cast<T*>(c.stage);
@@ -182,24 +167,12 @@ struct LogisticFn {
     team_sync(c.team);
   }
 
-  // 4 values per lane of feature i of this warp's chunk: shared memory (solver warp) or Tensor Memory (helper)
+  // 4 values per lane of features i0 .. i0 + NF - 1 of this warp's chunk (solver warp: chunk 0, helper: chunk 1)
   template <bool kHelper, int NF>
   __device__ __forceinline__ void load_features(const EvalCtx& c, int i0, T (&x)[NF][4]) const {
-    if constexpr (kHelper) {
-      uint32_t r[NF][4];
+    const T* X = static_cast<const T*>(c.stage) + kX + (kHelper ? 128 : 0) + 4 * c.lane;
 #pragma unroll
-      for (int q = 0; q < NF; ++q) tmem_ldx4_issue(c.tmem + (uint32_t)((i0 + q) * 4), r[q]);
-      tmem_wait_ldx4_groups<NF>(r);
-#pragma unroll
-      for (int q = 0; q < NF; ++q)
-#pragma unroll
-        for (int t = 0; t < 4; ++t) x[q][t] = __uint_as_float(r[q][t]);
-    } else {
-      const T* X0 = static_cast<const T*>(c.stage) + kX0;
-#pragma unroll
-      for (int q = 0; q < NF; ++q)
-        P4::get(*reinterpret_cast<const typename P4::type*>(X0 + (i0 + q) * 128 + 4 * c.lane), x[q]);
-    }
+    for (int q = 0; q < NF; ++q) P4::get(*reinterpret_cast<const typename P4::type*>(X + (i0 + q) * N), x[q]);
   }
   // margins z_j = sum_i Xt[i][j] w_i (i ascending) of the 4 samples this lane owns in its warp's chunk.  The chain
   // starts from -0: (-0) + p is p for every float p, the zeros with their signs included, so the first step leaves the
@@ -327,23 +300,15 @@ struct LogisticFn {
   __device__ __noinline__ void helper(const EvalCtx& c) const {
     T* xc = xchg(c);
     const int lane = c.lane;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(static_cast<T*>(c.stage) + kBar);
+    uint32_t parity = 0;
     for (;;) {
       team_sync(c.team);
       const int cmd = cmd_word(c)[0];
       if (cmd == kCmdExit) break;
-      if (cmd == kCmdStage) {
-        volatile int* cw = cmd_word(c);
-        const unsigned long long inst = (unsigned long long)(uint32_t)cw[1] | ((unsigned long long)(uint32_t)cw[2] << 32);
-        const T* src = data + (long long)inst * stride + 128 + 4 * lane;
-#pragma unroll 4
-        for (int i = 0; i < D; i += 2) {
-          T v[8];
-          P4::get(__ldg(reinterpret_cast<const typename P4::type*>(src + i * N)), &v[0]);
-          P4::get(__ldg(reinterpret_cast<const typename P4::type*>(src + (i + 1) * N)), &v[4]);
-          tmem_st8f(c.tmem + (uint32_t)(i * 4), v);
-        }
-        tmem_wait_st();
-        team_sync(c.team);
+      if (cmd == kCmdStage) {  // the next instance's block: wait until it has landed
+        mbar_wait(bar, parity);
+        parity ^= 1u;
         continue;
       }
       T z[4], coef[4];

@@ -1,5 +1,5 @@
 // cno_newton.cuh -- batched NewtonDescent<F>::Minimize, one warp per instance,
-// whole Solver::Minimize loop in one persistent kernel (sm_100a).
+// whole Solver::Minimize loop in one persistent kernel (sm_90a).
 //
 // Reference path (include/cppoptlib/...):
 //   solver/solver.h:181-224          Minimize loop (incl. the re-evaluation of a
@@ -10,7 +10,7 @@
 //                                    lower bound on alpha)
 //   solver/progress.h:153-327        Progress::Update
 //
-// B200 design: the per-instance Hessian block ([A | b] of the dense-quadratic
+// Design: the per-instance Hessian block ([A | b] of the dense-quadratic
 // family: 32.5 KB at d=64 fp64) is staged into the warp's shared-memory slice by
 // ONE TMA bulk copy (cp.async.bulk + mbarrier complete_tx), twice per iteration:
 // once as the LU workspace, once (unshifted) for the Armijo slope and the trial
@@ -139,132 +139,18 @@ struct SmemRowVec {
   }
 };
 
-// ---- the augmented matrix [H | rhs]: shared memory, or shared memory + Tensor Memory ----
+// ---- the augmented matrix [H | rhs] in the warp's shared-memory slice ----
 // Column-major, lane l owns rows l*E .. l*E+E-1 of every column.  For D = 64 fp64
-// the matrix alone is 32 KB per instance, which would cap an SM at 6 resident
-// warps; the elimination is a 64-step dependent chain per instance (latency
-// bound), so resident warps are what buys throughput.  Columns D/2 .. D-1 are
-// therefore kept in the warp's Tensor Memory window (a column = this lane's 2
-// doubles = 4 TMEM columns; tcgen05.ld/st .32x32b.x4) and only columns 0 .. D/2-1
-// and the right-hand side stay in shared memory: 17 KB per instance -> 13 warps/SM.
-// An entry of the pivot row is broadcast from shared memory (one LDS) or, for a
-// TMEM column, from the owner lane's registers (SHFL).  The arithmetic and its
-// order are unchanged.
-#ifdef CNO_WARP_EMULATION  // tests/emu: Tensor Memory as a host array of the emulated warp
-__device__ __forceinline__ void tmem_st2(uint32_t taddr, const double (&v)[2]) {
-  const uint32_t w[4] = {(uint32_t)__double2loint(v[0]), (uint32_t)__double2hiint(v[0]), (uint32_t)__double2loint(v[1]),
-                         (uint32_t)__double2hiint(v[1])};
-  emu::tmem_store(taddr, w, 4);
-}
-__device__ __forceinline__ void tmem_ld2_issue(uint32_t taddr, uint32_t (&r)[4]) { emu::tmem_load(taddr, r, 4); }
-template <int NG>
-__device__ __forceinline__ void tmem_ld2_wait(uint32_t (&r)[NG][4], double (&v)[NG][2]) {
-  for (int g = 0; g < NG; ++g) {
-    v[g][0] = __hiloint2double((int)r[g][1], (int)r[g][0]);
-    v[g][1] = __hiloint2double((int)r[g][3], (int)r[g][2]);
-  }
-}
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) { emu::tmem_load(taddr, r, 32); }
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t (&r)[32], double (&v)[8][2]) {
-  for (int t = 0; t < 8; ++t) {
-    v[t][0] = __hiloint2double((int)r[4 * t + 1], (int)r[4 * t]);
-    v[t][1] = __hiloint2double((int)r[4 * t + 3], (int)r[4 * t + 2]);
-  }
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const double (&v)[8][2]) {
-  uint32_t r[32];
-  for (int t = 0; t < 8; ++t) {
-    r[4 * t] = (uint32_t)__double2loint(v[t][0]);
-    r[4 * t + 1] = (uint32_t)__double2hiint(v[t][0]);
-    r[4 * t + 2] = (uint32_t)__double2loint(v[t][1]);
-    r[4 * t + 3] = (uint32_t)__double2hiint(v[t][1]);
-  }
-  emu::tmem_store(taddr, r, 32);
-}
-#else
-__device__ __forceinline__ void tmem_st2(uint32_t taddr, const double (&v)[2]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr),
-               "r"(__double2loint(v[0])), "r"(__double2hiint(v[0])), "r"(__double2loint(v[1])),
-               "r"(__double2hiint(v[1]))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld2_issue(uint32_t taddr, uint32_t (&r)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr)
-               : "memory");
-}
-template <int NG>
-__device__ __forceinline__ void tmem_ld2_wait(uint32_t (&r)[NG][4], double (&v)[NG][2]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int g = 0; g < NG; ++g) {
-    asm volatile("" : "+r"(r[g][0]), "+r"(r[g][1]), "+r"(r[g][2]), "+r"(r[g][3]));
-    v[g][0] = __hiloint2double((int)r[g][1], (int)r[g][0]);
-    v[g][1] = __hiloint2double((int)r[g][3], (int)r[g][2]);
-  }
-}
-
-// 8 matrix columns (= 32 TMEM columns) in one instruction
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t (&r)[32], double (&v)[8][2]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) asm volatile("" : "+r"(r[i]));
-#pragma unroll
-  for (int t = 0; t < 8; ++t) {
-    v[t][0] = __hiloint2double((int)r[4 * t + 1], (int)r[4 * t]);
-    v[t][1] = __hiloint2double((int)r[4 * t + 3], (int)r[4 * t + 2]);
-  }
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const double (&v)[8][2]) {
-  uint32_t r[32];
-#pragma unroll
-  for (int t = 0; t < 8; ++t) {
-    r[4 * t] = (uint32_t)__double2loint(v[t][0]);
-    r[4 * t + 1] = (uint32_t)__double2hiint(v[t][0]);
-    r[4 * t + 2] = (uint32_t)__double2loint(v[t][1]);
-    r[4 * t + 3] = (uint32_t)__double2hiint(v[t][1]);
-  }
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-      "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-      "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-#endif  // CNO_WARP_EMULATION
-
+// the matrix alone is 32 KB per instance: 6 resident warps per SM.
 template <class T, int D>
 struct AugStore {
   static constexpr int E = Shape<D>::E;
-  static constexpr bool kSplit = (sizeof(T) == 8 && D == 64);
-  static constexpr int kSm = kSplit ? D / 2 : D;   // matrix columns kept in shared memory
-  static constexpr int kTmemCols = kSplit ? (D - kSm) * 4 : 0;
   using RV = SmemRowVec<T, D>;
-  T* sm;        // [kSm matrix columns | rhs], each D rows
-  uint32_t tm;  // Tensor Memory window (kSplit)
+  T* sm;        // [D matrix columns | rhs], each D rows
   int lane;
 
-  __device__ __forceinline__ T* rhs() const { return sm + kSm * D; }
+  __device__ __forceinline__ T* rhs() const { return sm + D * D; }
   __device__ __forceinline__ T* smcol(int j) const { return sm + j * D; }
-  __device__ __forceinline__ uint32_t tmcol(int j) const { return tm + (uint32_t)((j - kSm) * 4); }
 };
 
 // ---- Second-mode device functors ------------------------------------------------
@@ -284,26 +170,11 @@ __device__ __forceinline__ void aug_gemv(const AugStore<T, D>& A, const T* vec, 
 #pragma unroll
   for (int e = 0; e < E; ++e) out[e] = col[e] * v0;
 #pragma unroll 4
-  for (int j = 1; j < AS::kSm; ++j) {
+  for (int j = 1; j < D; ++j) {
     AS::RV::load(A.smcol(j), A.lane, col);
     const T vj = vec[j];
 #pragma unroll
     for (int e = 0; e < E; ++e) out[e] = out[e] + col[e] * vj;
-  }
-  if constexpr (AS::kSplit) {
-#pragma unroll 1
-    for (int j0 = AS::kSm; j0 < D; j0 += 8) {
-      uint32_t r[32];
-      double c2[8][2];
-      tmem_ld32_issue(A.tmcol(j0), r);
-      tmem_ld32_wait(r, c2);
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        const T vj = vec[j0 + t];
-#pragma unroll
-        for (int e = 0; e < E; ++e) out[e] = out[e] + c2[t][e] * vj;
-      }
-    }
   }
 }
 
@@ -375,29 +246,18 @@ struct DenseQuadraticFn {
   const T* data;        // [B, stride]
   long long stride;     // scalars per instance (>= D*D + D)
 
-  // [A | b] -> the warp's store: shared-memory columns and b by TMA bulk copies
-  // (cp.async.bulk + mbarrier), Tensor Memory columns by coalesced loads + tcgen05.st
+  // [A | b] -> the warp's store by TMA bulk copies (cp.async.bulk + mbarrier)
   __device__ __forceinline__ void stage(const EvalCtx& c, const T (&)[E], const AS& A, uint64_t* bar,
                                         uint32_t& parity) const {
-    static_assert((AS::kSm * D * sizeof(T)) % 16 == 0 && (D * sizeof(T)) % 16 == 0,
+    static_assert((D * D * sizeof(T)) % 16 == 0 && (D * sizeof(T)) % 16 == 0,
                   "bulk copy sizes must be multiples of 16 bytes");
     const T* src = data + c.instance * stride;
     __syncwarp();
     if (c.lane == 0) {
       fence_proxy_async();  // order prior generic-proxy accesses of the store before the async writes
-      mbar_expect_tx(bar, (uint32_t)((AS::kSm * D + D) * sizeof(T)));
-      tma_bulk_g2s(A.sm, src, (uint32_t)(AS::kSm * D * sizeof(T)), bar);
+      mbar_expect_tx(bar, (uint32_t)((D * D + D) * sizeof(T)));
+      tma_bulk_g2s(A.sm, src, (uint32_t)(D * D * sizeof(T)), bar);
       tma_bulk_g2s(A.rhs(), src + D * D, (uint32_t)(D * sizeof(T)), bar);
-    }
-    if constexpr (AS::kSplit) {
-#pragma unroll 1
-      for (int j = AS::kSm; j < D; j += 8) {
-        double v[8][2];
-#pragma unroll
-        for (int t = 0; t < 8; ++t) load_row<T, D>(src + (j + t) * D, c.lane, v[t]);
-        tmem_st32(A.tmcol(j), v);
-      }
-      tmem_wait_st();
     }
     mbar_wait(bar, parity);
     parity ^= 1u;
@@ -513,7 +373,7 @@ template <class T, int D>
 struct NewtonSmem {
   static constexpr int E = Shape<D>::E;
   using AS = AugStore<T, D>;
-  static constexpr int kAug = D * (AS::kSm + 1);                 // [shared-memory columns | rhs]
+  static constexpr int kAug = D * (D + 1);                       // [matrix columns | rhs]
   static constexpr int kVecPad = ((D + 3) / 4) * 4;
   // + vec, ring, mbarrier (8 bytes); slice size kept a multiple of 16 bytes so every
   // warp's base stays aligned for 16-byte vector accesses and TMA bulk copies
@@ -522,8 +382,7 @@ struct NewtonSmem {
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
   static constexpr int kMaxSmem = 227 * 1024;
   static constexpr int kWarpsFit = (int)(kMaxSmem / kWarpBytes);
-  // Tensor Memory: 512 columns per lane quadrant / kTmemCols per warp
-  static constexpr int kCap = AS::kSplit ? 4 * (512 / AS::kTmemCols) : 8;
+  static constexpr int kCap = 8;
   static constexpr int kWarps = kWarpsFit > kCap ? kCap : (kWarpsFit < 1 ? 1 : kWarpsFit);
 };
 
@@ -579,72 +438,14 @@ __device__ __forceinline__ void lu_update_smem(const AugStore<T, D>& A, int j0, 
   }
 }
 
-// The same over the TENSOR-MEMORY columns k+1 .. D-1 (and at least kSm): the pivot
-// row's entry comes from its owner lane's registers (SHFL) instead of a
-// shared-memory broadcast.  Columns move in aligned groups of 8 (one
-// tcgen05.ld/st .x32 each); in a group that straddles column k only the columns
-// beyond k are touched.  PE = which of the owner lane's two rows is the pivot row.
-template <int D, int PE, bool kPartial>
-__device__ __forceinline__ void lu_update_tmem_group(const AugStore<double, D>& A, int j, int k, int owner,
-                                                     const double (&l)[2], const bool (&live)[2]) {
-  uint32_t r[32];
-  double cj[8][2];
-  tmem_ld32_issue(A.tmcol(j), r);
-  tmem_ld32_wait(r, cj);
-#pragma unroll
-  for (int t = 0; t < 8; ++t) {
-    const double u = __shfl_sync(kFullMask, cj[t][PE], owner);
-    const bool on = !kPartial || (j + t > k);
-#pragma unroll
-    for (int e = 0; e < 2; ++e)
-      if (on && live[e]) cj[t][e] = cj[t][e] - l[e] * u;
-  }
-  tmem_st32(A.tmcol(j), cj);
-}
-template <int D, int PE>
-__device__ __forceinline__ void lu_update_tmem(const AugStore<double, D>& A, int k, int prow,
-                                               const double (&l)[2], const bool (&live)[2]) {
-  constexpr int kSm = AugStore<double, D>::kSm;
-  const int owner = prow >> 1;
-  const int jfirst = (k + 1 > kSm) ? k + 1 : kSm;
-  int j = kSm + ((jfirst - kSm) & ~7);
-  if (j != jfirst) {  // uniform
-    lu_update_tmem_group<D, PE, true>(A, j, k, owner, l, live);
-    j += 8;
-  }
-#pragma unroll 1
-  for (; j < D; j += 8) lu_update_tmem_group<D, PE, false>(A, j, k, owner, l, live);
-  tmem_wait_st();
-}
-
-// this lane's rows of matrix column k, wherever the column lives
+// this lane's rows of matrix column k
 template <class T, int D>
 __device__ __forceinline__ void aug_load_col(const AugStore<T, D>& A, int k, T (&col)[Shape<D>::E]) {
-  using AS = AugStore<T, D>;
-  if constexpr (AS::kSplit) {
-    if (k >= AS::kSm) {  // uniform
-      uint32_t r[1][4];
-      double c2[1][2];
-      tmem_ld2_issue(A.tmcol(k), r[0]);
-      tmem_ld2_wait<1>(r, c2);
-      col[0] = c2[0][0];
-      col[1] = c2[0][1];
-      return;
-    }
-  }
-  AS::RV::load(A.smcol(k), A.lane, col);
+  AugStore<T, D>::RV::load(A.smcol(k), A.lane, col);
 }
 template <class T, int D>
 __device__ __forceinline__ void aug_store_col(const AugStore<T, D>& A, int k, const T (&col)[Shape<D>::E]) {
-  using AS = AugStore<T, D>;
-  if constexpr (AS::kSplit) {
-    if (k >= AS::kSm) {
-      tmem_st2(A.tmcol(k), col);
-      tmem_wait_st();
-      return;
-    }
-  }
-  AS::RV::store(A.smcol(k), A.lane, col);
+  AugStore<T, D>::RV::store(A.smcol(k), A.lane, col);
 }
 
 // Any Second-mode functor (value/gradient through operator()(ctx, x, grad*), Hessian column by column
@@ -894,17 +695,7 @@ __device__ __forceinline__ void lu_solve_inplace(const AugStore<T, D>& A, T (&de
     }
     aug_store_col<T, D>(A, k, col);
     // ---- trailing update, columns k+1 .. D-1 and the right-hand side ----
-    if (k + 1 < AS::kSm) {
-      lu_update_smem<T, D>(A, k + 1, AS::kSm, prow, l, live, A.rhs());
-    } else {
-      lu_update_smem<T, D>(A, AS::kSm, AS::kSm, prow, l, live, A.rhs());  // rhs only
-    }
-    if constexpr (AS::kSplit) {
-      if (k + 1 < D) {
-        if (prow & 1) lu_update_tmem<D, 1>(A, k, prow, l, live);  // uniform
-        else lu_update_tmem<D, 0>(A, k, prow, l, live);
-      }
-    }
+    lu_update_smem<T, D>(A, k + 1, D, prow, l, live, A.rhs());  // (k = D - 1: the rhs only)
     __syncwarp();
   }
   T rv[E];
@@ -933,23 +724,7 @@ newton_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   T* const ring = vec + SMN::kVecPad;
   uint64_t* const bar = reinterpret_cast<uint64_t*>(ring + CNO_MAX_PAST);
   uint32_t parity = 0;
-  uint32_t tmem_base = 0;
-#ifndef CNO_WARP_EMULATION  // (tests/emu: the emulated warp's Tensor Memory window starts at column 0)
-  if constexpr (AS::kSplit) {
-    __shared__ uint32_t tmem_base_s;
-    if (warp == 0) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                       (uint32_t)__cvta_generic_to_shared(&tmem_base_s)),
-                   "n"(512));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    tmem_base = tmem_base_s;
-  }
-#endif
-  const AS A{aug, tmem_base + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((warp >> 2) * AS::kTmemCols), lane};
+  const AS A{aug, lane};
   if (lane == 0) {
     mbar_init(bar, 1);
 #ifndef CNO_WARP_EMULATION
@@ -1009,25 +784,8 @@ newton_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         const int row = lane * E + e;
         if (row < D) {
           A.rhs()[row] = -g[e];
-          if (!AS::kSplit || row < AS::kSm) A.smcol(row)[row] += T(1e-5);
+          A.smcol(row)[row] += T(1e-5);
         }
-      }
-      if constexpr (AS::kSplit) {  // diagonal entries held in Tensor Memory
-#pragma unroll 1
-        for (int j0 = AS::kSm; j0 < D; j0 += 8) {
-          uint32_t r8[32];
-          double c8[8][2];
-          tmem_ld32_issue(A.tmcol(j0), r8);
-          tmem_ld32_wait(r8, c8);
-#pragma unroll
-          for (int t = 0; t < 8; ++t) {
-#pragma unroll
-            for (int e = 0; e < E; ++e)
-              if (lane * E + e == j0 + t) c8[t][e] = c8[t][e] + 1e-5;
-          }
-          tmem_st32(A.tmcol(j0), c8);
-        }
-        tmem_wait_st();
       }
       __syncwarp();
       lu_solve_inplace<T, D>(A, delta, vpos);
@@ -1106,13 +864,6 @@ newton_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     }
     __syncwarp();
   }
-#ifndef CNO_WARP_EMULATION
-  if constexpr (AS::kSplit) {
-    __syncthreads();  // every warp is done with its TMEM window
-    if (warp == 0)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-  }
-#endif
 }
 
 // ---- Progress::condition_hessian on request (solver/progress.h:203-210) ------------------------------------------
@@ -1126,7 +877,7 @@ newton_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
 // l*E2 .. l*E2+E2-1 (in-lane binary tree), then the cross-lane policy sum.
 //   D = 64: a lane's coefficients are two whole columns; a column's tree is the owner lanes' in-lane pairs followed by
 //           an ASCENDING xor butterfly (1, 2, 4, 8, 16 = the binary tree over the column's 64 rows), so columns are
-//           reduced where they live (shared memory, Tensor Memory or the registers of a solve) -- no d*d scratch;
+//           reduced where they live (shared memory or the registers of a solve) -- no d*d scratch;
 //   else:   the inverse is written to a d*d shared-memory scratch and both matrices are read linearly.
 template <class T, int D>
 struct ConditionSmem {
@@ -1168,23 +919,7 @@ condition_hessian_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ xs
   uint64_t* const bar = reinterpret_cast<uint64_t*>(ring + CNO_MAX_PAST);
   T* const inv = aug + SMN::kWarpElems;  // (kInv scalars; not used when kColumnwise)
   uint32_t parity = 0;
-  uint32_t tmem_base = 0;
-#ifndef CNO_WARP_EMULATION
-  if constexpr (AS::kSplit) {
-    __shared__ uint32_t tmem_base_s;
-    if (warp == 0) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                       (uint32_t)__cvta_generic_to_shared(&tmem_base_s)),
-                   "n"(512));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    tmem_base = tmem_base_s;
-  }
-#endif
-  const AS A{aug, tmem_base + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((warp >> 2) * AS::kTmemCols), lane};
+  const AS A{aug, lane};
   if (lane == 0) {
     mbar_init(bar, 1);
 #ifndef CNO_WARP_EMULATION
@@ -1271,13 +1006,6 @@ condition_hessian_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ xs
     if (lane == 0) out[b] = csqrt(part_h) * csqrt(part_i);
     __syncwarp();
   }
-#ifndef CNO_WARP_EMULATION
-  if constexpr (AS::kSplit) {
-    __syncthreads();
-    if (warp == 0)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-  }
-#endif
 }
 
 }  // namespace cno

@@ -1,6 +1,6 @@
 // cno_newton_dmma.cuh -- NewtonDescent<F>::Minimize for d = 64 fp64 with the dense
 // factorisation on the FP64 TENSOR CORE (policy CNO_POLICY_DMMA_LU), one warp per
-// instance, whole Solver::Minimize loop in one persistent kernel (sm_100a).
+// instance, whole Solver::Minimize loop in one persistent kernel (sm_90a).
 //
 // Reference path: solver/newton_descent.h:66-81 (H += 1e-5 I; delta = H.lu().solve(-g);
 // Armijo<F,2>), linesearch/armijo.h:82-101, solver/solver.h:181-224, solver/progress.h:153-327.
@@ -11,7 +11,7 @@
 // path follows the default fp64 specification.  An element of the trailing matrix receives
 //   a = fma(-l_i0, u_0j, a); a = fma(-l_i1, u_1j, a); ...        (pivot index ascending)
 // and mma.sync.m8n8k4.f64 evaluates exactly such a chain (d = c; d = fma(a_k, b_k, d), k = 0..3:
-// measured bit for bit on B200, tools/dmma_probe.cu).  So the elimination is BLOCKED here -- panels
+// tools/dmma_probe.cu checks this bit for bit on the GPU).  So the elimination is BLOCKED here -- panels
 // of 4 pivots; per panel: (1) the 64 x 4 panel is factored in registers (pivot search, division,
 // fused updates; the right-hand side rides along), (2) the row exchanges are applied to the matrix,
 // (3) the 4 pivot rows of the trailing block are finished (U12: three fused steps inside each
@@ -19,18 +19,14 @@
 // as one DMMA.8x8x4 per 8 x 8 tile with A = the NEGATED multipliers (that is how they are stored) --
 // and the result equals the UNBLOCKED fused elimination of the oracle bit for bit.
 //
-// STORAGE (two stores, both used inside one CTA; the factorisation is written against the concept):
+// STORAGE (the factorisation is written against the store concept below):
 //   SmemMat  the warp's shared-memory slice in TENSOR-CORE FRAGMENT ORDER: 64 tiles of 8 x 8 (tile (R, Cg) = rows 8R..,
 //            columns 8Cg.. at (8R + Cg) * 512 bytes); inside a tile row a = i % 8 owns four 16-byte slots (column
 //            pairs), slot 4a + (q ^ ((a >> 1) & 3)), halves exchanged in odd tile rows.  Lane 4a + q of a DMMA holds
 //            C[a][2q], C[a][2q+1]: one conflict-free LDS.128 / STS.128 per tile and lane; the XORs spread the rows of one
 //            COLUMN over the bank groups for the panel / substitution code (lane l owns rows 2l, 2l+1).  33.6 KB per
-//            instance.
-//   TmemMat  the same tiles as DMMA C fragments in TENSOR MEMORY (256 columns per warp); a whole tile row moves with
-//            one tcgen05.ld / st .32x32b.x32; cross-lane traffic through two 2.3 KB shared-memory panels.  5.4 KB of
-//            shared memory per instance.
-// 8 Tensor-Memory warps + 4 shared-memory warps per SM (NewtonDmmaSmem<3>); the right-hand side, the row permutation
-// and the solution stay in registers.  DESIGN.md 2.3b.
+//            instance: 6 warps per SM (NewtonDmmaSmem).
+// The right-hand side, the row permutation and the solution stay in registers.  DESIGN.md 2.3b.
 #ifndef CNO_NEWTON_DMMA_CUH_
 #define CNO_NEWTON_DMMA_CUH_
 
@@ -84,7 +80,7 @@ struct FragStore {
 };
 
 // ---- the matrix store, in shared memory ----------------------------------------------------------------
-// Concept (SmemMat here, TmemMat below; lu_dmma_factor / _back / _forward are written against it):
+// Concept (lu_dmma_factor / _back / _forward are written against it):
 //   stage(src, shift)            A (global, col-major, bitwise symmetric) + shift I -> the store
 //   panel_load(kb, P)            P[e][c] = element (2 lane + e, kb + c)
 //   swap_rows(k, p)              exchange two whole rows
@@ -94,7 +90,6 @@ struct FragStore {
 struct SmemMat {
   double* m;  // fragment order, FragStore
   int lane;
-  static constexpr bool kMaskedUpdate = false;  // one update<NCG> per number of live column groups
 
   // A is bitwise symmetric, so COLUMN j read from global memory (lane l: rows 2l, 2l+1 -- one coalesced 16-byte
   // load) is ROW j, columns 2l, 2l+1: exactly one 16-byte slot of the fragment order.
@@ -218,250 +213,6 @@ struct SmemMat {
       const double u2 = __shfl_sync(kFullMask, b[t], base + 2);
       if (r4 > 2) b[t] = cfma(nl2, u2, b[t]);
     }
-  }
-};
-
-// ---- the matrix store, in Tensor Memory ---------------------------------------------------------------------
-// The same 8 x 8 tiles, but a tile IS a DMMA C fragment in Tensor Memory: tile (R, cg) = 4 columns at 32 R + 4 cg of
-// the warp's window (256 columns = the whole matrix), TMEM lane 4a + q holding elements (8R + a, 8cg + 2q), (., + 1).
-// The trailing update then moves a whole TILE ROW (8 tiles) with ONE tcgen05.ld / tcgen05.st .32x32b.x32.  Tensor
-// Memory is lane-locked, so everything that crosses lanes goes through two small shared-memory panels:
-//   pbuf [4][72]  the current panel, column-major (rows' entries, the A fragments, the 4 x 4 diagonal block)
-//   ubuf [4][72]  the panel's four pivot rows across all 64 columns (U12, in and out of the B-fragment layout)
-// (together also the 8 x 72 staging area of one tile row) -- 5.4 KB of shared memory per instance instead of
-// 33.6 KB, which is what lets 8 such warps sit beside 5 shared-memory ones on an SM.  A row exchange moves two tile
-// rows through registers with shuffles (rare for the diagonally dominant Hessians of the benchmark).
-struct TmemMat {
-  uint32_t tm;   // window: lane quadrant in bits 31:16, first column in bits 15:0
-  double* pbuf;  // [4][kLd]; ubuf = pbuf + 4 * kLd
-  int lane;
-  static constexpr int kLd = 72;
-  static constexpr int kScratch = 8 * kLd;
-  __device__ __forceinline__ double* ubuf() const { return pbuf + 4 * kLd; }
-  __device__ __forceinline__ uint32_t tile(int R, int cg) const { return tm + (uint32_t)(32 * R + 4 * cg); }
-
-  __device__ __forceinline__ void row_load(int R, double (&v)[8][2]) const {
-    uint32_t r[32];
-    tmem_ld32_issue(tile(R, 0), r);
-    tmem_ld32_wait(r, v);
-  }
-  __device__ __forceinline__ void row_store(int R, const double (&v)[8][2]) const { tmem_st32(tile(R, 0), v); }
-  // the 8 tiles of column group cg (one per tile row)
-  __device__ __forceinline__ void col_load(int cg, double (&t)[8][2]) const {
-    uint32_t r[8][4];
-#pragma unroll
-    for (int R = 0; R < 8; ++R) tmem_ld2_issue(tile(R, cg), r[R]);
-    tmem_ld2_wait<8>(r, t);
-  }
-
-  // one tile row at a time: 8 coalesced rows -> the 8 x 72 scratch -> fragment order -> tcgen05.st
-  __device__ __forceinline__ void stage(const double* __restrict__ src, double shift, const double* xv,
-                                        double (&ax)[2]) const {
-    double* const sc = pbuf;
-    const int a = lane >> 2, q = lane & 3;
-#pragma unroll 1
-    for (int R = 0; R < 8; ++R) {
-      double v[8][2];
-#pragma unroll
-      for (int t = 0; t < 8; ++t) load_row<double, 64>(src + (8 * R + t) * 64, lane, v[t]);
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {  // A xv on the way (see SmemMat::stage)
-        const int j = 8 * R + t;
-        const double xj = xv[j];
-        ax[0] = (j == 0) ? (v[t][0] * xj) : (ax[0] + v[t][0] * xj);
-        ax[1] = (j == 0) ? (v[t][1] * xj) : (ax[1] + v[t][1] * xj);
-      }
-      __syncwarp();
-#pragma unroll
-      for (int t = 0; t < 8; ++t) st2(sc + t * kLd + 2 * lane, v[t][0], v[t][1]);
-      __syncwarp();
-      double w[8][2];
-#pragma unroll
-      for (int cg = 0; cg < 8; ++cg) {
-        const double2 d = ld2(sc + a * kLd + 8 * cg + 2 * q);
-        w[cg][0] = d.x;
-        w[cg][1] = d.y;
-      }
-      // the diagonal elements of this tile row: (8R + a, 8R + a) = tile (R, R), lane 4a + a/2, element a % 2
-#pragma unroll
-      for (int cg = 0; cg < 8; ++cg) {
-        if (cg == R && q == (a >> 1)) {
-          if (a & 1) w[cg][1] = w[cg][1] + shift;
-          else w[cg][0] = w[cg][0] + shift;
-        }
-      }
-      row_store(R, w);
-    }
-    tmem_wait_st();
-    __syncwarp();
-  }
-  __device__ __forceinline__ void panel_load(int kb, double (&P)[2][4]) const {
-    const int cgk = kb >> 3, q0 = (kb & 7) >> 1;
-    const int a = lane >> 2, q = lane & 3;
-    double t[8][2];
-    col_load(cgk, t);
-    __syncwarp();  // (pbuf may still be read by the lanes' previous step)
-    if (q == q0 || q == q0 + 1) {
-      double* const c0 = pbuf + (2 * (q - q0)) * kLd + a;
-#pragma unroll
-      for (int R = 0; R < 8; ++R) {
-        c0[8 * R] = t[R][0];
-        c0[kLd + 8 * R] = t[R][1];
-      }
-    }
-    __syncwarp();
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const double2 d = ld2(pbuf + c * kLd + 2 * lane);
-      P[0][c] = d.x;
-      P[1][c] = d.y;
-    }
-  }
-  // (a real call: rare, and four inlined copies per panel would crowd the instruction cache)
-  __device__ __noinline__ void swap_rows(int k, int p) const {
-    if (lane < 4) {  // the panel being factored lives in pbuf: its rows move too
-      double* const c = pbuf + lane * kLd;
-      const double t = c[k];
-      c[k] = c[p];
-      c[p] = t;
-    }
-    const int Rk = k >> 3, Rp = p >> 3, a = lane >> 2;
-    const int sk = 4 * (k & 7) + (lane & 3), sp = 4 * (p & 7) + (lane & 3);
-    const bool isk = a == (k & 7), isp = a == (p & 7);
-    double va[8][2];
-    row_load(Rk, va);
-    if (Rk == Rp) {  // uniform
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const double fp = __shfl_sync(kFullMask, va[i][e], sp), fk = __shfl_sync(kFullMask, va[i][e], sk);
-          va[i][e] = isk ? fp : (isp ? fk : va[i][e]);
-        }
-      }
-      row_store(Rk, va);
-    } else {
-      double vb[8][2];
-      row_load(Rp, vb);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const double fp = __shfl_sync(kFullMask, vb[i][e], sp), fk = __shfl_sync(kFullMask, va[i][e], sk);
-          if (isk) va[i][e] = fp;
-          if (isp) vb[i][e] = fk;
-        }
-      }
-      row_store(Rk, va);
-      row_store(Rp, vb);
-    }
-    tmem_wait_st();
-  }
-  // a finished panel column goes to the panel buffer (column-major: rows 2 lane, 2 lane + 1 are one 16-byte slot)
-  __device__ __forceinline__ void panel_col_store(int j, double v0, double v1) const {
-    st2(pbuf + (j & 3) * kLd + 2 * lane, v0, v1);
-  }
-  // the factored panel (pbuf, rows already exchanged) back into the tiles of its column group
-  __device__ __forceinline__ void panel_commit(int kb) const {
-    const int cgk = kb >> 3, q0 = (kb & 7) >> 1;
-    const int a = lane >> 2, q = lane & 3;
-    double t[8][2];
-    col_load(cgk, t);  // (after the row exchanges: the other four columns of the group moved with their rows)
-    __syncwarp();
-    if (q == q0 || q == q0 + 1) {
-      const double* const c0 = pbuf + (2 * (q - q0)) * kLd + a;
-#pragma unroll
-      for (int R = 0; R < 8; ++R) {
-        t[R][0] = c0[8 * R];
-        t[R][1] = c0[kLd + 8 * R];
-      }
-    }
-#pragma unroll
-    for (int R = 0; R < 8; ++R) tmem_st2(tile(R, cgk), t[R]);
-    tmem_wait_st();
-  }
-  __device__ __forceinline__ void diag(int kb, double (&d)[4][4]) const {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {  // (column-major panel: rows kb .. kb+3 of a column are 32 contiguous bytes)
-      const double2 lo = ld2(pbuf + c * kLd + kb), hi = ld2(pbuf + c * kLd + kb + 2);
-      d[0][c] = lo.x; d[1][c] = lo.y; d[2][c] = hi.x; d[3][c] = hi.y;
-    }
-  }
-  // Two variants cover all panels (the instruction cache holds both stores' code): NG = 8 or 4 column groups are
-  // processed, of which the first `cgl - (8 - NG)` are no longer live (cgl = the first live group, run time) -- their
-  // products are computed and dropped, a tile row costs one tcgen05.ld / st regardless.
-  static constexpr bool kMaskedUpdate = true;
-  template <int NG>
-  __device__ __forceinline__ void update(int kb) const {
-    constexpr int cg0 = 8 - NG;
-    const int r4 = lane & 3, n8 = lane >> 2;  // (also: n8 = this lane's row inside a tile, r4 = its column pair)
-    const bool part = (kb & 7) == 0;
-    const int ka = kb & 7, Rk = kb >> 3;
-    const int cgl = (kb + 4) >> 3;  // first live column group = first live tile row (partial when `part`)
-    double* const ub = ubuf();
-    __syncwarp();  // pbuf holds the factored panel
-    const double nl0 = pbuf[kb + r4], nl1 = pbuf[kLd + kb + r4], nl2 = pbuf[2 * kLd + kb + r4];
-    // live[t]: this lane's two columns of group cg0 + t take the update (the first live group only from column kb+4 on)
-    bool live[NG], ulive[NG];
-#pragma unroll
-    for (int t = 0; t < NG; ++t) {
-      live[t] = (cg0 + t > cgl) || (cg0 + t == cgl && (!part || r4 >= 2));
-      ulive[t] = (cg0 + t > cgl) || (cg0 + t == cgl && (!part || n8 >= 4));  // same, for a B-fragment lane (column n8)
-    }
-    // ---- (3) U12 through ubuf: the pivot rows' lanes publish them, the B-fragment lanes solve, and back ----
-    double v[8][2];
-    row_load(Rk, v);
-    const bool prow_lane = (n8 >= ka) && (n8 < ka + 4);
-    double* const mine = ub + (n8 - ka) * kLd + 2 * r4;
-    if (prow_lane) {
-#pragma unroll
-      for (int t = 0; t < NG; ++t) st2(mine + 8 * (cg0 + t), v[cg0 + t][0], v[cg0 + t][1]);
-    }
-    __syncwarp();
-    double bfrag[NG];
-    double* const bsrc = ub + r4 * kLd + n8;
-#pragma unroll
-    for (int t = 0; t < NG; ++t) bfrag[t] = bsrc[8 * (cg0 + t)];
-    SmemMat::u12_solve<NG>(bfrag, nl0, nl1, nl2, r4, lane & ~3);
-#pragma unroll
-    for (int t = 0; t < NG; ++t)
-      if (r4 > 0 && ulive[t]) bsrc[8 * (cg0 + t)] = bfrag[t];
-    __syncwarp();
-    if (prow_lane) {
-#pragma unroll
-      for (int t = 0; t < NG; ++t) {
-        const double2 d = ld2(mine + 8 * (cg0 + t));
-        v[cg0 + t][0] = d.x;
-        v[cg0 + t][1] = d.y;
-      }
-    }
-    // ---- (4) the trailing update, a tile row per tcgen05.ld / st ----
-    const double* const asrc = pbuf + r4 * kLd + n8;  // A fragment of tile row R: (8R + n8, kb + r4)
-    if (part) {  // uniform: the pivot rows' tile row also holds the live rows kb+4 .. kb+7
-      const double afrag = asrc[8 * Rk];
-#pragma unroll
-      for (int t = 0; t < NG; ++t) {
-        double d0, d1;
-        dmma(d0, d1, afrag, bfrag[t], v[cg0 + t][0], v[cg0 + t][1]);
-        if (n8 >= 4 && live[t]) { v[cg0 + t][0] = d0; v[cg0 + t][1] = d1; }
-      }
-    }
-    row_store(Rk, v);
-#pragma unroll 1
-    for (int R = Rk + 1; R < 8; ++R) {
-      const double afrag = asrc[8 * R];
-      double w[8][2];
-      row_load(R, w);
-#pragma unroll
-      for (int t = 0; t < NG; ++t) {
-        double d0, d1;
-        dmma(d0, d1, afrag, bfrag[t], w[cg0 + t][0], w[cg0 + t][1]);
-        if (live[t]) { w[cg0 + t][0] = d0; w[cg0 + t][1] = d1; }
-      }
-      row_store(R, w);
-    }
-    tmem_wait_st();
-    __syncwarp();
   }
 };
 
@@ -589,20 +340,15 @@ __device__ __forceinline__ void lu_dmma_factor(const Mat& M, double (&rv)[2], in
     if (kb == 60) break;
 
     // ---- (3) U12 and (4) the trailing update: straight-line code per number of (processed) column groups ----
-    if constexpr (Mat::kMaskedUpdate) {
-      if (kb + 4 >= 32) M.template update<4>(kb);
-      else M.template update<8>(kb);
-    } else {
-      switch (8 - ((kb + 4) >> 3)) {
-        case 8: M.template update<8>(kb); break;
-        case 7: M.template update<7>(kb); break;
-        case 6: M.template update<6>(kb); break;
-        case 5: M.template update<5>(kb); break;
-        case 4: M.template update<4>(kb); break;
-        case 3: M.template update<3>(kb); break;
-        case 2: M.template update<2>(kb); break;
-        default: M.template update<1>(kb); break;
-      }
+    switch (8 - ((kb + 4) >> 3)) {
+      case 8: M.template update<8>(kb); break;
+      case 7: M.template update<7>(kb); break;
+      case 6: M.template update<6>(kb); break;
+      case 5: M.template update<5>(kb); break;
+      case 4: M.template update<4>(kb); break;
+      case 3: M.template update<3>(kb); break;
+      case 2: M.template update<2>(kb); break;
+      default: M.template update<1>(kb); break;
     }
   }
   __syncwarp();
@@ -717,23 +463,13 @@ __device__ __forceinline__ void prefetch_block_l2(const double* block, int lane)
 #endif
 }
 
-// Warp populations of a CTA (kLayout): which store each warp's instance lives in.
-//   0: 6 warps, matrices in shared memory                      (33.6 KB each)
-//   1: 8 warps, matrices in Tensor Memory                      (256 columns + 5.4 KB of shared memory each)
-//   2: 13 warps: warps 0..7 Tensor Memory, warps 8..12 shared memory -- both stores full, 13 instances in flight
-//      (one sub-partition then hosts 4 warps: 128 registers per thread)
-//   3: 12 warps: 8 Tensor Memory + 4 shared memory (3 warps per sub-partition: 168 registers per thread)
-//   4: 10 warps: 4 Tensor Memory + 6 shared memory
-template <int kLayout>
+// The CTA: 6 warps, each with its matrix (33.6 KB) and vectors in its shared-memory slice.
 struct NewtonDmmaSmem {
   static constexpr int kVecElems = 128 /*two vectors*/ + 32 /*64 ints*/ + CNO_MAX_PAST;
-  static constexpr int kSmemWarpElems = FragStore::kElems + kVecElems;
-  static constexpr int kTmemWarpElems = TmemMat::kScratch + kVecElems;
-  static_assert(kSmemWarpElems % 2 == 0 && kTmemWarpElems % 2 == 0, "warp slices stay 16-byte aligned");
-  static constexpr int kTmemWarps = kLayout == 0 ? 0 : (kLayout == 4 ? 4 : 8);
-  static constexpr int kSmemWarps = kLayout == 0 ? 6 : (kLayout == 1 ? 0 : (kLayout == 2 ? 5 : (kLayout == 3 ? 4 : 6)));
-  static constexpr int kWarps = kTmemWarps + kSmemWarps;
-  static constexpr size_t kBytes = ((size_t)kTmemWarps * kTmemWarpElems + (size_t)kSmemWarps * kSmemWarpElems) * sizeof(double);
+  static constexpr int kWarpElems = FragStore::kElems + kVecElems;
+  static_assert(kWarpElems % 2 == 0, "warp slices stay 16-byte aligned");
+  static constexpr int kWarps = 6;
+  static constexpr size_t kBytes = (size_t)kWarps * kWarpElems * sizeof(double);
   static_assert(kBytes <= 227 * 1024, "shared memory per CTA");
 };
 
@@ -748,7 +484,7 @@ __device__ __forceinline__ void newton_dmma_warp(const Fn& fn, const Mat& M, dou
   constexpr int E = 2;
   using AS = AugStore<T, D>;
   const int lane = M.lane;
-  const AS none{nullptr, 0u, lane};  // (the functor's evaluations read global memory, not a staged block)
+  const AS none{nullptr, lane};  // (the functor's evaluations read global memory, not a staged block)
 
   // The work queue is read ONE INSTANCE AHEAD: while instance b is being solved, the block of the instance this warp
   // takes next is already on its way into L2.
@@ -760,8 +496,9 @@ __device__ __forceinline__ void newton_dmma_warp(const Fn& fn, const Mat& M, dou
     if (uni(b >= (unsigned long long)batch)) break;
     if (lane == 0) bnext = atomicAdd(queue, 1ULL);
     bnext = __shfl_sync(kFullMask, bnext, 0);
-    // (the prefetch itself is issued after the first iteration, see below: with two blocks per warp in flight for the
-    // whole solve the 12 x 148 warps' footprint reaches the L2's size and the second and third pass over A miss)
+    // (the prefetch itself is issued after the first iteration, see below: with two 33 KB blocks per warp in flight for
+    // the whole solve, 6 warps x 132 SMs come to about 52 MB -- the size of the 50 MB L2 -- and the second and third
+    // pass over A would miss)
     const EvalCtx ctx{lane, (long long)b, nullptr};
 
     T x[E], g[E];
@@ -872,55 +609,21 @@ __device__ __forceinline__ void newton_dmma_warp(const Fn& fn, const Mat& M, dou
   }
 }
 
-template <class Fn, int kLayout>
-__global__ void __launch_bounds__(NewtonDmmaSmem<kLayout>::kWarps * 32, 1)
+template <class Fn>
+__global__ void __launch_bounds__(NewtonDmmaSmem::kWarps * 32, 1)
 newton_dmma_minimize_kernel(const Fn fn, const double* __restrict__ x0, const long long batch,
                             const StopParams<double> stop, const BatchOut<double> out,
                             unsigned long long* __restrict__ queue) {
   static_assert(Fn::Dim == 64 && sizeof(typename Fn::Scalar) == 8 && Fn::kHessianConstant,
                 "the tensor-core factorisation is instantiated for constant 64 x 64 fp64 Hessians");
-  using SMN = NewtonDmmaSmem<kLayout>;
+  using SMN = NewtonDmmaSmem;
   CNO_DYNAMIC_SMEM(smem_raw);
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
-  double* const smem = reinterpret_cast<double*>(smem_raw);
-  uint32_t tmem_base = 0;
-#ifndef CNO_WARP_EMULATION  // (tests/emu: the emulated warp's Tensor Memory window starts at column 0)
-  if constexpr (SMN::kTmemWarps > 0) {
-    __shared__ uint32_t tmem_base_s;
-    if (warp == 0) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                       (uint32_t)__cvta_generic_to_shared(&tmem_base_s)),
-                   "n"(512));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    tmem_base = tmem_base_s;
-  }
-#endif
-  bool tmem_warp = SMN::kTmemWarps > 0;  // (a compile-time constant for the one-store populations)
-  if constexpr (SMN::kTmemWarps > 0 && SMN::kSmemWarps > 0) tmem_warp = uni(warp < SMN::kTmemWarps);
-  if (tmem_warp) {  // warp w may touch TMEM lanes 32 (w % 4) .. +31; two windows of 256 columns per quadrant
-    double* const base = smem + (size_t)warp * SMN::kTmemWarpElems;
-    double* const vec = base + TmemMat::kScratch;
-    const TmemMat M{tmem_base + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((warp >> 2) * 256), base, lane};
-    newton_dmma_warp(fn, M, vec, reinterpret_cast<int*>(vec + 128), vec + 128 + 32, x0, batch, stop, out, queue);
-  } else {
-    double* const base = smem + (size_t)SMN::kTmemWarps * SMN::kTmemWarpElems +
-                         (size_t)(warp - SMN::kTmemWarps) * SMN::kSmemWarpElems;
-    double* const vec = base + FragStore::kElems;
-    const SmemMat M{base, lane};
-    newton_dmma_warp(fn, M, vec, reinterpret_cast<int*>(vec + 128), vec + 128 + 32, x0, batch, stop, out, queue);
-  }
-#ifndef CNO_WARP_EMULATION
-  if constexpr (SMN::kTmemWarps > 0) {
-    __syncthreads();  // every warp is done with its TMEM window
-    if (warp == 0)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-  }
-#endif
+  double* const base = reinterpret_cast<double*>(smem_raw) + (size_t)warp * SMN::kWarpElems;
+  double* const vec = base + FragStore::kElems;
+  const SmemMat M{base, lane};
+  newton_dmma_warp(fn, M, vec, reinterpret_cast<int*>(vec + 128), vec + 128 + 32, x0, batch, stop, out, queue);
 }
 
 }  // namespace cno

@@ -1,10 +1,10 @@
 /*
- * cno.h -- C ABI of the B200-native batched unconstrained-minimisation engine.
+ * cno.h -- C ABI of the H100-native batched unconstrained-minimisation engine.
  *
  * This is the drop-in boundary for ONE path of PatWie/CppNumericalSolvers
  * (cppoptlib 2.0.0): solver::{Lbfgs,Bfgs,NewtonDescent}::Minimize with the
  * MoreThuente / Armijo line searches and the Progress stopping rules, with a
- * batch axis added (B independent instances, one warp per instance on sm_100a).
+ * batch axis added (B independent instances, one warp per instance on sm_90a).
  *
  * Plain C: pointers and sizes only, no C++/torch types.  All citations are
  * relative to the reference tree (include/cppoptlib/...).

@@ -4,7 +4,7 @@
  *
  * Parity: the device path behind these entry points equals the pinned CPU oracle
  * (oracle/cno_al_oracle.h, tests/test_al_oracle.py) and the reference-headers
- * fixtures bit for bit on a B200 (tests/test_al_gpu.py).  DESIGN.md 8.
+ * fixtures bit for bit on the GPU (tests/test_al_gpu.py).  DESIGN.md 8.
  *
  * Reference interfaces replaced (include/cppoptlib/...):
  *   solver/augmented_lagrangian.h:63-239    AugmentedLagrangianConfig   cno_al_config_t

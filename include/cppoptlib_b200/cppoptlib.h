@@ -806,7 +806,7 @@ template <class F> class ConjugatedGradientDescent : public Solver<F, CNO_CONJUG
 
 
 // ---- the constrained caller of the path (solver/augmented_lagrangian.h, function_problem.h) ----
-// Parity: tests/cpp/al_host.cc, run on a B200 by tests/test_al_gpu.py.
+// Parity: tests/cpp/al_host.cc, run on the GPU by tests/test_al_gpu.py.
 }  // namespace solver
 
 namespace function {

@@ -1,6 +1,6 @@
 // cppoptlib_b200/device.cuh -- compile a USER objective (or a composite of objectives) for the device.
 //
-// In an nvcc translation unit (-gencode arch=compute_100a,code=sm_100a -fmad=false, include path =
+// In an nvcc translation unit (-gencode arch=compute_90a,code=sm_90a -fmad=false, include path =
 // cppnumericalsolvers_b200/csrc; include THIS header before any other cppoptlib_b200 header):
 //
 //   struct MyF : cppoptlib::function::FunctionCRTP<MyF, double, First, 64> {

@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real GPU, an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session", autouse=True)
 def _built():
-    """Make sure libcno.so and the oracle exist (prebuilt on the GPU box)."""
+    """Make sure libcno.so and the oracle exist (normally built by __graft_entry__.build())."""
     from cppnumericalsolvers_b200 import _lib
     if not os.path.exists(_lib.LIB_PATH):
         from cppnumericalsolvers_b200 import build

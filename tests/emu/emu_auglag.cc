@@ -112,7 +112,6 @@ int run(const Obj& obj, int op, const cno_constraints_t* k, long long B, const E
   if (op == kInner) {
     // the fused inner solve: lbfgs_minimize_kernel<AugLagFn<Obj>> exactly as al_run launches it
     // (x0 = state x, out.x = x_work, out.nfev = inner_nfev), one emulated warp draining the queue.
-    // (shapes whose y-history lives in Tensor Memory -- fp64, d = 128 -- use the host array of warp_emu.h)
     {
       const cno::AugLagFn<Obj> fn{obj, v};
       const cno_stop_t* inner = static_cast<const cno_stop_t*>(x_in);
@@ -201,7 +200,7 @@ extern "C" int emu_minimize(int solver, int hager_zhang, const cno_problem_t* p,
   return CNO_ERR_UNSUPPORTED;
 }
 
-// NewtonDescent (csrc/cno_newton.cuh) under emulation: the TMA bulk copy is a memcpy, Tensor Memory a host array.
+// NewtonDescent (csrc/cno_newton.cuh) under emulation: the TMA bulk copy is a memcpy.
 template <class Fn>
 int run_newton(const Fn& fn, long long B, const void* x0, const cno_stop_t* stop, const cno_batch_out_t* out) {
   using T = typename Fn::Scalar;
@@ -221,18 +220,12 @@ extern "C" int emu_newton(const cno_problem_t* p, long long batch, const void* x
     cno::DenseQuadraticDmmaFn fn;
     fn.data = static_cast<const double*>(p->data);
     fn.stride = (long long)p->data_stride;
-    // p->n selects the store the emulated warp uses: 0 = shared memory, 1 = Tensor Memory (a host array here)
     unsigned long long queue = 0;
-    const int layout = p->n;
     emu::run_warp([&](int lane) {
       blockIdx.x = 0;
       threadIdx.x = (unsigned)lane;
-      if (layout == 1)
-        cno::newton_dmma_minimize_kernel<cno::DenseQuadraticDmmaFn, 1>(fn, (const double*)x0, batch, cno::make_stop<double>(*stop),
-                                                                      cno::make_out<double>(*out), &queue);
-      else
-        cno::newton_dmma_minimize_kernel<cno::DenseQuadraticDmmaFn, 0>(fn, (const double*)x0, batch, cno::make_stop<double>(*stop),
-                                                                      cno::make_out<double>(*out), &queue);
+      cno::newton_dmma_minimize_kernel<cno::DenseQuadraticDmmaFn>(fn, (const double*)x0, batch, cno::make_stop<double>(*stop),
+                                                                  cno::make_out<double>(*out), &queue);
     });
     return 0;
   }
@@ -284,7 +277,7 @@ extern "C" int emu_condition_hessian(const cno_problem_t* p, long long batch, co
 }
 
 // L-BFGS on the logistic-regression functor (csrc/cno_logistic.cuh: per-instance data staged by TMA into shared
-// memory and by tcgen05.st into Tensor Memory) under emulation.
+// memory) under emulation.
 extern "C" int emu_logistic(const cno_problem_t* p, long long batch, const void* x0, const cno_stop_t* stop,
                             const cno_batch_out_t* out) {
   if (!(p->family == CNO_FN_LOGISTIC && p->dtype == CNO_F32 && p->d == 64 && p->n == 256)) return CNO_ERR_UNSUPPORTED;
@@ -311,7 +304,7 @@ extern "C" int emu_logistic_evaluate(const cno_problem_t* p, long long batch, co
   const Fn fn{static_cast<const float*>(p->data), (long long)p->data_stride, (float)p->param};
   alignas(16) static float stage[Fn::kStageElems];
   emu::run_team([&](int lane, int w) {
-    cno::EvalCtx ctx{lane, 0, stage, 0u, 0};
+    cno::EvalCtx ctx{lane, 0, stage, 0};
     if (w == 1) { fn.helper(ctx); return; }
     uint32_t parity = 0;
     fn.init_stage(ctx);

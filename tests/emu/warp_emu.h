@@ -1,6 +1,6 @@
 // tests/emu/warp_emu.h -- HOST stand-ins for the CUDA warp intrinsics, so that device
-// source (csrc/*.cuh functors and the one-warp-per-instance kernels that do not need
-// Tensor Memory / TMA) can be executed on the CPU by 32 lock-step std::threads.
+// source (csrc/*.cuh functors and the one-warp-per-instance kernels, TMA copies as memcpy)
+// can be executed on the CPU by 32 lock-step std::threads.
 //
 // TEST INFRASTRUCTURE ONLY (like oracle/): it is how device code whose first GPU run is
 // still pending gets exercised against the oracle in the `-m "not gpu"` suite.  Nothing in
@@ -9,7 +9,7 @@
 //
 // Semantics: every collective is "publish my value -> barrier -> read -> barrier".  The
 // FP64 tensor-core reduction (mma.sync.m8n8k4.f64 with A = ones) is restated with the
-// arithmetic measured on B200 (tools/dmma_probe.cu): d = c; d = fma(1, b_k, d) = d + b_k.
+// arithmetic tools/dmma_probe.cu checks on the GPU: d = c; d = fma(1, b_k, d) = d + b_k.
 #ifndef CNO_WARP_EMU_H_
 #define CNO_WARP_EMU_H_
 
@@ -69,8 +69,6 @@ struct Warp {
   uint64_t slot[32];
   double dslot[32];
   double dslot2[32];
-  uint32_t tmem[32][512];  // Tensor Memory window of the emulated warp: [lane][column], 32-bit cells
-  uint32_t (*tm)[512] = tmem;   // the window this warp addresses (a helper warp of a team shares its leader's: same lane quadrant)
   SpinBarrier* team = nullptr;  // named barrier of a leader + helper team (bar.sync id, 64)
 };
 inline thread_local int tl_lane = 0;
@@ -124,16 +122,6 @@ inline void dmma(double& d0, double& d1, double a, double b, double c0, double c
   d1 = r1;
 }
 
-// tcgen05.st / tcgen05.ld .32x32b.xN: lane l moves N consecutive 32-bit columns of its own TMEM lane
-inline void tmem_store(uint32_t taddr, const uint32_t* w, int n) {
-  const uint32_t col = taddr & 0xffffu;
-  for (int i = 0; i < n; ++i) tl_warp->tm[tl_lane][col + i] = w[i];
-}
-inline void tmem_load(uint32_t taddr, uint32_t* w, int n) {
-  const uint32_t col = taddr & 0xffffu;
-  for (int i = 0; i < n; ++i) w[i] = tl_warp->tm[tl_lane][col + i];
-}
-
 // Runs f(lane) on 32 lock-step threads = one warp.
 inline void run_warp(const std::function<void(int)>& f) {
   static Warp w_storage;  // (one emulated warp at a time; too large for the stack)
@@ -151,8 +139,8 @@ inline void run_warp(const std::function<void(int)>& f) {
 // bar.sync id, 64: the two warps of a team meet (all 64 threads arrive)
 inline void team_sync() { tl_warp->team->arrive_and_wait(); }
 
-// Runs f(lane, w) on 64 lock-step threads = a leader warp (w = 0) and its helper warp (w = 1), which share the leader's
-// Tensor Memory window and a named barrier; shared memory is the kernel's function-static array, as for one warp.
+// Runs f(lane, w) on 64 lock-step threads = a leader warp (w = 0) and its helper warp (w = 1), which share a named
+// barrier; shared memory is the kernel's function-static array, as for one warp.
 inline void run_team(const std::function<void(int, int)>& f) {
   static Warp w_storage[2];
   static SpinBarrier team_bar;
@@ -160,7 +148,6 @@ inline void run_team(const std::function<void(int, int)>& f) {
   team_bar.total = 64;
   for (int w = 0; w < 2; ++w) {
     new (&w_storage[w]) Warp();
-    w_storage[w].tm = w_storage[0].tmem;
     w_storage[w].team = &team_bar;
   }
   std::vector<std::thread> ts;

@@ -1,6 +1,5 @@
 """AugmentedLagrangian on the device (include/cno_al.h, csrc/cno_auglag.cuh) against the pinned CPU
-oracle and the reference-headers fixtures tests/golden/al_*.npz, bit for bit (first green B200 run:
-round 2, gpurun_out/r02_al_first.log)."""
+oracle and the reference-headers fixtures tests/golden/al_*.npz, bit for bit."""
 import glob
 import os
 

@@ -4,13 +4,13 @@ csrc/cno_auglag.cuh (the composite functor AugLagFn and the auto-scale / outer-s
 kernels) and the solver kernels (csrc/cno_lbfgs.cuh, cno_bfgs.cuh, cno_descent.cuh with
 cno_linesearch.cuh) are compiled by g++ against tests/emu/warp_emu.h -- 32 lock-step threads per
 warp, the warp intrinsics as publish/barrier/read, the FP64 tensor-core reduction restated with the
-arithmetic measured on B200 -- and driven through the outer loop of csrc/cno_api.cu::al_run,
+arithmetic of tools/dmma_probe.cu -- and driven through the outer loop of csrc/cno_api.cu::al_run,
 restated here in numpy.  The inner solve is either the oracle's L-BFGS on the composite or the fused
 device kernel itself under emulation.  Everything must equal the oracle -- which equals the
 reference's own headers -- bit for bit; the GPU-validated kernels are run too, to show that the
-emulation reproduces what the B200 computes.
+emulation reproduces what the GPU computes.
 
-The same paths run on a B200 in tests/test_al_gpu.py; this is their `-m "not gpu"` counterpart."""
+The same paths run on the GPU in tests/test_al_gpu.py; this is their `-m "not gpu"` counterpart."""
 import ctypes as C
 import glob
 import os
@@ -212,8 +212,7 @@ def test_emulated_device_loop_known_answers(emu):
 @pytest.mark.parametrize("family,dtype,d,n_eq", [(ob.FN_ROSENBROCK, np.float64, 128, 1), (ob.FN_ROSENBROCK, np.float32, 8, 1)])
 def test_emulated_device_loop_with_the_device_inner_kernel(emu, family, dtype, d, n_eq):
     """lbfgs_minimize_kernel<AugLagFn<Obj>> (with its active() skip of finished instances) + the outer-loop
-    kernels, all device source, all under emulation == the oracle, bit for bit (d = 128: the y-history of
-    the inner kernel lives in the emulated Tensor Memory)."""
+    kernels, all device source, all under emulation == the oracle, bit for bit."""
     B = 2  # 32 lock-step threads per warp: a few instances keep this to seconds
     rng = np.random.default_rng(300 + d)
     x0 = ob.fill_uniform((B, d), 0, 57 + d, -1.5, 1.5, dtype)
@@ -232,13 +231,13 @@ SOLVER_KEYS = ("num_iterations", "status", "nfev", "x", "value", "gradient", "x_
 
 @pytest.mark.parametrize("solver,hz,dtype,d,limit", [
     (ob.LBFGS, 0, np.float64, 2, 10000), (ob.LBFGS, 0, np.float64, 37, 40), (ob.LBFGS, 0, np.float32, 37, 20),
-    (ob.LBFGS, 0, np.float64, 128, 50), (ob.LBFGS, 1, np.float64, 128, 25),  # the headline shape: y-history in (emulated) Tensor Memory
+    (ob.LBFGS, 0, np.float64, 128, 50), (ob.LBFGS, 1, np.float64, 128, 25),  # the headline shape
     (ob.LBFGS, 1, np.float64, 8, 10000), (ob.BFGS, 0, np.float64, 8, 10000), (ob.BFGS, 1, np.float64, 2, 10000),
     (ob.GRADIENT_DESCENT, 0, np.float64, 8, 40), (ob.GRADIENT_DESCENT, 1, np.float64, 8, 40),
     (ob.CONJUGATED_GRADIENT_DESCENT, 0, np.float64, 8, 8)])
 def test_emulation_reproduces_gpu_validated_kernels(emu, solver, hz, dtype, d, limit):
     """The L-BFGS / BFGS / descent kernels (MoreThuente and HagerZhang) are bit-identical to the oracle on the
-    B200; run under the emulation they must be too -- that is what makes the emulated AugmentedLagrangian
+    GPU; run under the emulation they must be too -- that is what makes the emulated AugmentedLagrangian
     results above evidence about the device code rather than about the emulator."""
     B = 2
     x0 = ob.fill_uniform((B, d), 0, 900 + d, -2.0, 2.0, dtype)
@@ -333,8 +332,7 @@ def _spd_data(B, d, seed, dtype=np.float64):
 @pytest.mark.parametrize("family,dtype,d", [(ob.FN_DENSE_QUADRATIC, np.float64, 64), (ob.FN_DENSE_QUADRATIC, np.float32, 64),
                                             (ob.FN_DENSE_QUADRATIC, np.float64, 12), (ob.FN_ROSENBROCK, np.float64, 2)])
 def test_emulation_reproduces_the_newton_kernel(emu, family, dtype, d):
-    """newton_minimize_kernel under emulation (the TMA bulk copy as a memcpy, the Tensor Memory half of the d = 64
-    fp64 matrix as a host array) == the oracle, as on the B200."""
+    """newton_minimize_kernel under emulation (the TMA bulk copy as a memcpy) == the oracle, as on the GPU."""
     B = 2
     x0 = ob.fill_uniform((B, d), 0, 5, -2.0, 2.0, dtype)
     data = _spd_data(B, d, 9, dtype) if family == ob.FN_DENSE_QUADRATIC else None
@@ -392,10 +390,10 @@ def _newton_pivot_cases(d=64, B=8):
     return np.ascontiguousarray(np.concatenate([A.transpose(0, 2, 1).reshape(B, -1), bvec], axis=1))
 
 
-@pytest.mark.parametrize("store", ["shared_memory", "tensor_memory"])
+@pytest.mark.parametrize("store", ["shared_memory"])
 @pytest.mark.parametrize("case", ["spd", "pivoting", "huge", "tiny"])
 def test_emulation_tensor_core_newton_equals_the_fused_oracle(emu, case, store):
-    """csrc/cno_newton_dmma.cuh (CNO_POLICY_DMMA_LU) under emulation, DMMA.8x8x4 as the FMA chain measured on B200:
+    """csrc/cno_newton_dmma.cuh (CNO_POLICY_DMMA_LU) under emulation, DMMA.8x8x4 as the FMA chain of tools/dmma_probe.cu:
     the BLOCKED elimination (register panels, U12 in the B-fragment layout, tensor-core trailing update, blocked
     substitutions) equals the oracle's UNBLOCKED lu_solve with fused multiply-subtracts bit for bit."""
     d = 64
@@ -405,9 +403,8 @@ def test_emulation_tensor_core_newton_equals_the_fused_oracle(emu, case, store):
         data = _newton_pivot_cases(d) * {"pivoting": 1.0, "huge": 1e150, "tiny": 1e-150}[case]
         B = data.shape[0]
     x0 = ob.fill_uniform((B, d), 0, 5, -2.0, 2.0, np.float64)
-    # (the harness reads the store of the emulated warp from the problem's n field: the matrix in shared memory in
-    # fragment order, or in Tensor Memory -- a host array under emulation -- with the small shared-memory panels)
-    prob = ob.Problem(ob.FN_DENSE_QUADRATIC, ob._np_dtype(x0), d, 1 if store == "tensor_memory" else 0, 0.0,
+    # (the matrix lives in the emulated warp's shared memory, in fragment order)
+    prob = ob.Problem(ob.FN_DENSE_QUADRATIC, ob._np_dtype(x0), d, 0, 0.0,
                       data.ctypes.data, data.shape[1], ob.POLICY_DMMA_LU, 0)
     stop = ob.default_stop()
     stop.num_iterations = 4
@@ -431,9 +428,8 @@ def test_emulation_tensor_core_newton_equals_the_fused_oracle(emu, case, store):
 
 
 def test_emulation_reproduces_the_logistic_kernel(emu):
-    """L-BFGS on the logistic-regression functor (csrc/cno_logistic.cuh): per-instance data staged by TMA bulk
-    copies into shared memory and by tcgen05.st into Tensor Memory -- under emulation a memcpy and a host array --
-    and evaluated by a TEAM of two warps (solver warp + helper warp, 64 lock-step threads meeting at the named
+    """L-BFGS on the logistic-regression functor (csrc/cno_logistic.cuh): per-instance data staged by a TMA bulk
+    copy into shared memory -- under emulation a memcpy -- and evaluated by a TEAM of two warps (solver warp + helper warp, 64 lock-step threads meeting at the named
     barrier; emu::run_team).  Three instances through one team: the data are re-staged and the helper re-armed."""
     B, n, d, lam = 3, 256, 64, 1e-2
     rng = np.random.default_rng(3)

@@ -135,7 +135,7 @@ def sweep_al(trials=24):
 
 def sweep_newton(trials=24):
     """NewtonDescent on dense quadratics: well-conditioned, nearly singular, indefinite, rank-deficient,
-    NaN / Inf entries -- the pivoted LU with the shared-memory / Tensor Memory split (d = 64 fp64) and without."""
+    NaN / Inf entries -- the pivoted LU at d = 64 fp64 and at other shapes."""
     rng = np.random.default_rng(31)
     n = bad_n = 0
     for trial in range(trials):

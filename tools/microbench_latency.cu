@@ -1,4 +1,4 @@
-// tools/microbench_latency.cu -- dependent-issue latencies on sm_100a that bound
+// tools/microbench_latency.cu -- dependent-issue latencies on the GPU that bound
 // the one-warp-per-instance reduction chain (DADD, DMUL, SHFL.BFLY b32 pair, LDS).
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,12 +1,12 @@
 """tools/ncu_source_stalls.py -- per-source-line warp-stall breakdown of one kernel from an ncu capture.
 
-   cuobjdump -xelf all cppnumericalsolvers_b200/libcno.so && nvdisasm -gi cno_api.sm_100a.cubin > gi.txt
+   cuobjdump -xelf all cppnumericalsolvers_b200/libcno.so && nvdisasm -gi cno_api.sm_90a.cubin > gi.txt
    ncu -i prof.ncu-rep --page source --csv > source.csv          (capture made with --set full --import-source on)
    python tools/ncu_source_stalls.py gi.txt source.csv <mangled kernel name>
 
 Joins the SASS addresses of ncu's source page with nvdisasm's inline line info (innermost file:line per instruction) and
 prints, per source line, its share of all stall samples, the instructions executed (1e7) and the share of every stall
-reason in percent of ALL samples.  Used for DESIGN.md 2.4 (profiles/r02_c3_stall_attribution.txt)."""
+reason in percent of ALL samples.  Used for DESIGN.md 2.4."""
 import re, csv, collections, sys
 gi, src, fn = sys.argv[1:4]
 txt=open(gi).read().split('\n')

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """tools/ncu_summary.py <report.ncu-rep> [iterations] -- text summary of one ncu --set full
-capture (raw + source pages) for profiles/.  `iterations` = solver iterations executed by
+capture (raw + source pages).  `iterations` = solver iterations executed by
 the profiled launch (to normalise instruction counts)."""
 import collections
 import csv
@@ -75,10 +75,7 @@ def main():
         path = sys.argv[sys.argv.index("--mix-json") + 1]
         json.dump({"kernel": "lbfgs_minimize_kernel<RosenbrockFn<double,128>,10>", "report": rep,
                    "iterations_in_profiled_launch": iters, "instr_per_iteration": tot / iters,
-                   "fp64_per_iteration": fp64 / iters, "dmma_per_iteration": dmma / iters, "dmma_cycles": 16.0,
-                   "dmma_cycles_source": "tools/fp64_pipe_probe.cu on B200: DADD 2.0, DMMA.8x8x4 16.0 cycles per "
-                                         "warp instruction per SM sub-partition, and the two add up when mixed "
-                                         "(one shared FP64 datapath)"}, open(path, "w"), indent=1)
+                   "fp64_per_iteration": fp64 / iters, "dmma_per_iteration": dmma / iters}, open(path, "w"), indent=1)
 
 
 if __name__ == "__main__":

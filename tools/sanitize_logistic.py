@@ -1,5 +1,5 @@
 """tools/sanitize_logistic.py -- tiny run of the two-warps-per-instance logistic kernel (csrc/cno_logistic.cuh: named
-barriers, exchange buffers in shared memory, TMA-staged chunk, Tensor-Memory chunk), for compute-sanitizer.
+barriers, exchange buffers in shared memory, TMA-staged block), for compute-sanitizer.
    compute-sanitizer --tool racecheck python tools/sanitize_logistic.py"""
 import os
 import sys

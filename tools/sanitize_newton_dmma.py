@@ -1,6 +1,5 @@
-"""tools/sanitize_newton_dmma.py -- tiny runs of the tensor-core NewtonDescent kernel (every warp population: matrices in
-shared memory, in Tensor Memory, both) with row exchanges forced, and of the condition-number kernel, for
-compute-sanitizer.  Usage on the GPU box:  compute-sanitizer --tool racecheck python tools/sanitize_newton_dmma.py"""
+"""tools/sanitize_newton_dmma.py -- tiny runs of the tensor-core NewtonDescent kernel with row exchanges forced, and of the
+condition-number kernel, for compute-sanitizer.  Usage:  compute-sanitizer --tool racecheck python tools/sanitize_newton_dmma.py"""
 import os
 import sys
 
@@ -22,9 +21,7 @@ data = torch.from_numpy(np.concatenate([A.transpose(0, 2, 1).reshape(B, -1), rng
 p = cn.Progress(num_iterations=3, gradient_norm=1e-5, x_delta=1e-9, x_delta_violations=1, past=3, past_delta=1e-6)
 x0 = torch.empty(B, d, dtype=torch.float64, device=dev)
 cn.fill_uniform(x0, 0, 1, -2.0, 2.0)
-for layout in ("0", "1", "3"):
-    os.environ["CNO_NEWTON_DMMA_LAYOUT"] = layout
-    cn.NewtonDescent(p).Minimize(cn.DenseQuadratic(data, d, policy=_lib.POLICY_DMMA_LU), cn.BatchedFunctionState(x0))
+cn.NewtonDescent(p).Minimize(cn.DenseQuadratic(data, d, policy=_lib.POLICY_DMMA_LU), cn.BatchedFunctionState(x0))
 cn.ConditionHessian(cn.DenseQuadratic(data, d), x0)
 cn.ConditionHessian(cn.RosenbrockFull(8), x0[:, :8].contiguous())
 torch.cuda.synchronize()
