@@ -16,7 +16,7 @@
 //
 // Optional members the solver kernels look for (traits in cno_device.cuh):
 //   kStageElems + init_stage()/stage()  per-instance data staged into the warp's shared-memory slice (StageElems)
-//   kPreferredWarps                     resident warps per CTA the functor's register budget allows (FnPreferredWarps)
+//   kRegsPerThread                      registers per thread the plain L-BFGS kernel needs (FnRegsPerThread)
 //   active(instance)                    instances the kernel skips (FnSkipsInstances; AugLagFn)
 //   kHelperWarps = 1 + helper()/release_helper()   a second warp per instance that the functor drives through a
 //                                       named barrier (FnHelperWarps; LogisticFn, built-in functors only)
@@ -42,10 +42,10 @@ struct RosenbrockFn {
   static constexpr int E = Shape<D>::E;
 
   static constexpr bool kHasPartial = true;
-  // fp64, 4 elements per lane, default policy: the register budget allows 20 resident warps (cno_device.cuh:
-  // FnPreferredWarps).  Shared memory decides where the history is larger: at m = 10 (20 KiB per instance) 11 warps fit,
-  // at m = 5 the full 20.
-  static constexpr int kPreferredWarps = (sizeof(T) == 8 && E == 4 && std::is_same<P, PolicyFast>::value) ? 20 : 16;
+  // fp64, 4 elements per lane, default policy: 96 registers (20 warps where shared memory has room, as at m = 5).
+  // The kernel then spills a little (at m = 5: 88 bytes stored, 164 loaded per thread), and was measured faster on an
+  // H100 than 16 warps at 128 registers without spills (DESIGN.md 2.1).
+  static constexpr int kRegsPerThread = (sizeof(T) == 8 && E == 4 && std::is_same<P, PolicyFast>::value) ? 96 : 128;
   __device__ __forceinline__ T operator()(const EvalCtx& c, const T (&x)[E],
                                           T (*grad)[E]) const {
     return warp_sum_p<P, T, E>(partial(c, x, grad), RedCtx<T>{static_cast<T*>(c.stage), c.lane});

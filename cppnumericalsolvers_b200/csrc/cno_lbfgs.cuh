@@ -13,8 +13,8 @@
 // a global atomic queue (instances run 20..10000 iterations, so retire +
 // refill is what keeps all warps busy through the tail).  The m-deep (s, y)
 // history of the instance a warp is working on stays ON CHIP for the instance's
-// whole lifetime, in the warp's private slice of shared memory (at d = 128 fp64
-// that is 20 KB per instance: 11 resident warps per SM); x, g, the
+// whole lifetime, its newest pairs in registers and the rest in the warp's private slice of shared memory
+// (LbfgsPlan; at d = 128 fp64, m = 10: one pair in registers, 18 KB per instance, 12 resident warps per SM); x, g, the
 // search direction and the trial point live in registers.  HBM is touched twice
 // per instance: one coalesced vectorised read of x0 and one write of the result.
 // Inner products: in-lane tree, then the cross-lane sum on the FP64 tensor core
@@ -29,20 +29,33 @@
 #include "cno_linesearch.cuh"
 #include "cno_kernel_params.h"
 
+// Compile-time cap on the warps per CTA of every L-BFGS plan (default: none).  tools/lbfgs_warp_sweep.py builds
+// copies of the library with -DCNO_LBFGS_MAX_WARPS=w to measure throughput against resident warps.
+#ifndef CNO_LBFGS_MAX_WARPS
+#define CNO_LBFGS_MAX_WARPS 32
+#endif
+
 namespace cno {
 
-template <class T, int D, int M, int kStage = 0, int kScratchPerLane = 0, int kMaxW = 16, int kHelpers = 0>
+// The warp's shared-memory slice when the kRegPairs newest (s, y) pairs are held in registers and the older
+// M - kRegPairs in shared memory.
+template <class T, int D, int M, int kStage = 0, int kScratchPerLane = 0, int kMaxW = 16, int kHelpers = 0,
+          int kRegPairs_ = 0>
 struct LbfgsSmem {
   static constexpr int E = Shape<D>::E;
   static constexpr int kVec = 32 * E;                        // elements per stored vector
-  static constexpr int kScalars = 2 * M + CNO_MAX_PAST + 32 * kScratchPerLane;  // rho[M], alpha[M], f ring, policy scratch
-  static constexpr int kHistElems = 2 * M * kVec + ((kScalars + 3) / 4) * 4;  // S, Y + scalars
+  static constexpr int kRegPairs = kRegPairs_;
+  static constexpr int kSmemPairs = M - kRegPairs;           // slots of the shared ring
+  static_assert(kRegPairs >= 0 && kSmemPairs >= 1, "at least one pair lives in shared memory");
+  // rho and alpha of the shared pairs, f ring, policy scratch
+  static constexpr int kScalars = 2 * kSmemPairs + CNO_MAX_PAST + 32 * kScratchPerLane;
+  static constexpr int kHistElems = 2 * kSmemPairs * kVec + ((kScalars + 3) / 4) * 4;  // S, Y + scalars
   static constexpr int kWarpElems = kHistElems + kStage;     // + the functor's staged block
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
-  // warps per CTA: as many as fit in 227 KB, at most 16 (register budget).
+  // warps per CTA: as many as fit in 227 KB, at most kMaxW (register budget).
   static constexpr int kMaxSmem = 227 * 1024;
   static constexpr int kWarpsFit = (int)(kMaxSmem / kWarpBytes);
-  static constexpr int kMaxWarps = kMaxW;  // register budget: 65536 / (32 * warps) per thread (FnPreferredWarps)
+  static constexpr int kMaxWarps = kMaxW < CNO_LBFGS_MAX_WARPS ? kMaxW : CNO_LBFGS_MAX_WARPS;
   static constexpr int kWarps = kWarpsFit > kMaxWarps ? kMaxWarps : (kWarpsFit < 1 ? 1 : kWarpsFit);
   // Functors with a helper warp per instance (FnHelperWarps): solver warps 0 .. kWarps-1, the helper of solver warp t is
   // warp kHelperBase + t.
@@ -164,15 +177,46 @@ struct ResumeLayout {
   static constexpr size_t kBytes = ((kInts + kNumInts * sizeof(int) + 15) / 16) * 16;
 };
 
-// The shared-memory / warp plan of lbfgs_minimize_kernel<Fn, M, kResume, LS>.  The functor's preferred warp
-// count applies to the plain kernel only (MoreThuente, First mode, fused): the other variants carry more live
-// state per thread and keep the 128-register budget.
+// Most warps per CTA (one CTA per SM) whose per-thread register budget holds `regs`.  The warps are spread over the
+// SM's 4 sub-partitions, each with its own 16384-register file, and registers are allocated in units of 8 per
+// thread: the budget is 16384 / (32 ceil(W / 4)) rounded down to a multiple of 8 -- 168 up to 12 warps, 128 up to 16,
+// 96 up to 20 -- and ptxas's cap is 255.
+constexpr int lbfgs_register_warps(int regs) {
+  int w = 32;
+  while (w > 1 && ((16384 / (32 * ((w + 3) / 4))) & ~7) < regs) --w;
+  return regs > 255 ? 1 : w;
+}
+
+// The shared-memory / register / warp plan of lbfgs_minimize_kernel<Fn, M, kResume, LS>.  Shared memory holds the
+// history of one instance per warp; registers hold the functor's plain-kernel state (FnRegsPerThread) plus,
+// per pair kept in registers, 2 E values per lane.  Where shared memory limits the warp count, pairs held in the
+// registers the SM has spare make room for more warps: the plan takes the fewest register pairs (at most 2: each one
+// is unrolled code in both loops of the recursion) that reach the most warps, counting only warps that keep the
+// per-thread register budget of the kernel without register pairs (measured at d = 128 fp64, m = 10 on an H100:
+// 1 pair and 12 warps at 168 registers beat 2 pairs and 14 warps at 128, where the kernel spills).  Only the plain
+// kernel (MoreThuente, First mode, fused, no helper warp) does so: the other variants carry more live state per
+// thread and keep the 128-register budget and the whole history in shared memory (the stepwise record layout,
+// ResumeLayout, assumes it).
 template <class Fn, int M, bool kResume = false, class LS = LsMoreThuente>
 struct LbfgsPlan {
-  static constexpr bool kPlain = std::is_same<LS, LsMoreThuente>::value && !IsSecondMode<Fn>::value && !kResume;
-  using SM = LbfgsSmem<typename Fn::Scalar, Fn::Dim, M, StageElems<Fn>::value,
-                       PolicyScratch<typename PolicyOf<Fn>::type>::kElemsPerLane,
-                       kPlain ? FnPreferredWarps<Fn>::value : 16, FnHelperWarps<Fn>::value>;
+  using T = typename Fn::Scalar;
+  static constexpr bool kPlain = std::is_same<LS, LsMoreThuente>::value && !IsSecondMode<Fn>::value && !kResume &&
+                                 FnHelperWarps<Fn>::value == 0;
+  static constexpr int kRegs = kPlain ? FnRegsPerThread<Fn>::value : 128;
+  static constexpr int kPairRegs = 2 * Shape<Fn::Dim>::E * (int)(sizeof(T) / 4);
+  template <int R, int kCap>
+  using Smem = LbfgsSmem<T, Fn::Dim, M, StageElems<Fn>::value, PolicyScratch<typename PolicyOf<Fn>::type>::kElemsPerLane,
+                         kCap, FnHelperWarps<Fn>::value, R>;
+  static constexpr int kW0 = Smem<0, lbfgs_register_warps(kRegs)>::kWarps;
+  static constexpr int kSameBudget = 4 * ((kW0 + 3) / 4);  // most warps with the register budget of kW0 warps
+  template <int R>
+  using WithPairs = Smem<R, R == 0 ? lbfgs_register_warps(kRegs)
+                                   : (lbfgs_register_warps(kRegs + R * kPairRegs) < kSameBudget
+                                          ? lbfgs_register_warps(kRegs + R * kPairRegs) : kSameBudget)>;
+  static constexpr int kW1 = (kPlain && M > 1) ? WithPairs<(M > 1 ? 1 : 0)>::kWarps : 0;
+  static constexpr int kW2 = (kPlain && M > 2) ? WithPairs<(M > 2 ? 2 : 0)>::kWarps : 0;
+  static constexpr int kRegPairs = (kW2 > kW1 && kW2 > kW0) ? 2 : (kW1 > kW0 ? 1 : 0);
+  using SM = WithPairs<kRegPairs>;
 };
 
 template <class Fn, int M, bool kResume = false, class LS = LsMoreThuente>
@@ -190,6 +234,11 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   using SM = typename LbfgsPlan<Fn, M, kResume, LS>::SM;
   using SV = SmemVec<T, E>;
   constexpr T eps = Num<T>::eps;
+  // History split: the R newest pairs in registers, the MS = M - R older ones in the shared ring.
+  constexpr int R = SM::kRegPairs;
+  constexpr int MS = SM::kSmemPairs;
+  constexpr int RA = R > 0 ? R : 1;  // (extent of the register arrays)
+  static_assert(!kResume || R == 0, "the stepwise record holds the whole history in shared-memory slot order");
 
   CNO_DYNAMIC_SMEM(smem_raw);
   const int lane = threadIdx.x & 31;
@@ -198,11 +247,11 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   // the instance slot this warp works for: its own, or (helper warps) the one of its solver warp
   const int slot = (kHelpers > 0 && warp >= SM::kHelperBase) ? warp - SM::kHelperBase : warp;
   T* const S = reinterpret_cast<T*>(smem_raw) + (size_t)slot * SM::kWarpElems;
-  T* const rho_s = S + 2 * M * SM::kVec;  // 1 / (s_i . y_i) per slot
-  const YHist<T, E> Y{S + M * SM::kVec, lane};
+  T* const rho_s = S + 2 * MS * SM::kVec;  // 1 / (s_i . y_i) per slot
+  const YHist<T, E> Y{S + MS * SM::kVec, lane};
   typename YHist<T, E>::Pending ypend;
-  T* const alpha = rho_s + M;
-  T* const ring = alpha + M;
+  T* const alpha = rho_s + MS;
+  T* const ring = alpha + MS;
   // policy scratch (PolicyEigenSSE2): 16-byte aligned tail of the scalar block; handed to
   // functors through EvalCtx::stage when they stage nothing themselves
   T* const red_scratch = (PolicyScratch<P>::kElemsPerLane > 0) ? (ring + CNO_MAX_PAST) : nullptr;
@@ -233,8 +282,12 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     T x[E], g[E];
     T f;
     uint32_t nfev;
+    // mem_count pairs, chronological i = 0 (oldest) .. mem_count - 1.  Pair i lives in register slot
+    // mem_count - 1 - i if that is below R (rs/ry/rrho[0]: the newest), else in shared slot (mem_pos + i) mod MS;
+    // mem_pos stays 0 until the ring is full.  At R = 0 this is the reference's index map (lbfgs.h:162).
     int mem_count, mem_pos;
-    unsigned valid;  // bit idx set <=> !(|s_idx . y_idx| < eps)  (lbfgs.h:165,189)
+    unsigned valid;  // bit i set <=> !(|s_i . y_i| < eps), i chronological  (lbfgs.h:165,189)
+    T rs[RA][E], ry[RA][E], rrho[RA];
     T gamma;
     T xx;            // ||x||^2 carried across iterations (the dot the reference recomputes at lbfgs.h:95)
     ProgressState<T> prog;
@@ -319,20 +372,28 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       const int k = mem_count;
 
       // ================= two-loop recursion (:157-196) =====================
-      // chronological i -> slot (mem_pos + i) mod M; mem_pos stays 0 until the
-      // buffer is full, so this is the reference's index map (:162).  In both
-      // loops the loads of the next pair are issued before the current reduction
-      // (the reduction is the critical path; LDS latency hides under it).
+      // Pairs in chronological order (see mem_count): loop 1 takes the register pairs, then the shared ones;
+      // loop 2 the reverse.  In both loops the loads of the next shared pair are issued before the current
+      // reduction (the reduction is the critical path; LDS latency hides under it).
+      T ra[RA];  // alpha of the register pairs
       if (uni(k == M && valid == ((1u << M) - 1u))) {
         // ---- steady state (full history, every pair usable): both loops fully
         //      unrolled, alpha_i in registers, no per-pair control flow ----
-        int idx = mem_pos + M - 1;
-        idx = (idx >= M) ? idx - M : idx;
+        int idx = mem_pos + MS - 1;
+        idx = (idx >= MS) ? idx - MS : idx;
         T sv[E], yv[E];
-        SV::load(S + idx * SM::kVec, lane, sv);
+        if (R == 0) SV::load(S + idx * SM::kVec, lane, sv);
 #pragma unroll
-        for (int i = M - 1; i >= 0; --i) {  // first loop (:157-171): newest pair first
-          const int idx_next = (idx == 0) ? M - 1 : idx - 1;
+        for (int j = 0; j < R; ++j) {  // first loop (:157-171), register pairs: newest first
+          const auto part = lane_dot_p<P, T, E>(rs[j], q);
+          if (j + 1 == R) SV::load(S + idx * SM::kVec, lane, sv);
+          ra[j] = rrho[j] * warp_sum_p<P, T, E>(part, rc);
+#pragma unroll
+          for (int e = 0; e < E; ++e) q[e] = q[e] - ra[j] * ry[j][e];
+        }
+#pragma unroll
+        for (int i = MS - 1; i >= 0; --i) {  // first loop, shared pairs
+          const int idx_next = (idx == 0) ? MS - 1 : idx - 1;
           const auto part = lane_dot_p<P, T, E>(sv, q);
           const T r = rho_s[idx];
           Y.issue(idx, yv, ypend);
@@ -350,42 +411,60 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         idx = mem_pos;
         // (yv still holds y of the oldest pair: the last pair of loop 1 is the first of loop 2)
 #pragma unroll
-        for (int i = 0; i < M; ++i) {  // second loop (:185-196): oldest pair first
-          const int idx_next = (idx + 1 == M) ? 0 : idx + 1;
+        for (int i = 0; i < MS; ++i) {  // second loop (:185-196), shared pairs: oldest first
+          const int idx_next = (idx + 1 == MS) ? 0 : idx + 1;
           const auto part = lane_dot_p<P, T, E>(yv, q);
           const T r = rho_s[idx];
           const T al = alpha[i];
           SV::load(S + idx * SM::kVec, lane, sv);
-          if (i + 1 < M) Y.issue(idx_next, yv, ypend);
+          if (i + 1 < MS) Y.issue(idx_next, yv, ypend);
           const T beta = r * warp_sum_p<P, T, E>(part, rc);
           const T coef = al - beta;
 #pragma unroll
           for (int j = 0; j < E; ++j) q[j] = q[j] + sv[j] * coef;
-          if (i + 1 < M) Y.wait(yv, ypend);
+          if (i + 1 < MS) Y.wait(yv, ypend);
           idx = idx_next;
         }
+#pragma unroll
+        for (int j = R - 1; j >= 0; --j) {  // second loop, register pairs
+          const auto part = lane_dot_p<P, T, E>(ry[j], q);
+          const T beta = rrho[j] * warp_sum_p<P, T, E>(part, rc);
+          const T coef = ra[j] - beta;
+#pragma unroll
+          for (int e = 0; e < E; ++e) q[e] = q[e] + rs[j][e] * coef;
+        }
       } else {
-        // ---- warm-up (k < M) or a skipped pair: generic rolled loops ----
+        // ---- warm-up (k < M) or a skipped pair: the register pairs unrolled, the shared ones in rolled loops ----
+        const int kr = k < R ? k : R;  // pairs in registers
+        const int ks = k - kr;         // pairs in shared memory
         // ---- first loop (:157-171): newest pair first ----
-        // chronological i -> slot (mem_pos + i) mod M; mem_pos stays 0 until the
-        // buffer is full, so this is the reference's index map (:162).  The loads
-        // of the next pair are issued before the current reduction (software
-        // pipelining: the butterfly is the critical path, LDS latency hides under it).
-        if (uni(k > 0)) {
-          int idx = mem_pos + k - 1;
-          idx = (idx >= M) ? idx - M : idx;
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+          if (uni(j < kr)) {
+            const auto part = lane_dot_p<P, T, E>(rs[j], q);
+            const T a = rrho[j] * warp_sum_p<P, T, E>(part, rc);
+            if (uni((valid >> (k - 1 - j)) & 1u)) {  // lbfgs.h:165 skip
+              ra[j] = a;
+#pragma unroll
+              for (int e = 0; e < E; ++e) q[e] = q[e] - a * ry[j][e];
+            }
+          }
+        }
+        if (uni(ks > 0)) {
+          int idx = mem_pos + ks - 1;
+          idx = (idx >= MS) ? idx - MS : idx;
           T sv[E];
           SV::load(S + idx * SM::kVec, lane, sv);
   #pragma unroll 1
-          for (int i = k - 1; uni(i >= 0); --i) {
-            const int idx_next = (idx == 0) ? M - 1 : idx - 1;
+          for (int i = ks - 1; uni(i >= 0); --i) {
+            const int idx_next = (idx == 0) ? MS - 1 : idx - 1;
             const auto part = lane_dot_p<P, T, E>(sv, q);
             T yv[E];
             Y.issue(idx, yv, ypend);
             SV::load(S + idx_next * SM::kVec, lane, sv);  // prefetch (harmless at i == 0)
             const T a = rho_s[idx] * warp_sum_p<P, T, E>(part, rc);
             Y.wait(yv, ypend);
-            if (uni((valid >> idx) & 1u)) {  // lbfgs.h:165 skip
+            if (uni((valid >> i) & 1u)) {  // lbfgs.h:165 skip
               if (lane == 0) alpha[i] = a;
   #pragma unroll
               for (int j = 0; j < E; ++j) q[j] = q[j] - a * yv[j];
@@ -398,26 +477,38 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   #pragma unroll
         for (int j = 0; j < E; ++j) q[j] = kSecond ? (precond[j] * q[j]) : (q[j] * gamma);
         // ---- second loop (:185-196): oldest pair first ----
-        if (uni(k > 0)) {
+        if (uni(ks > 0)) {
           int idx = mem_pos;
           T yv[E];
           Y.issue(idx, yv, ypend);
           Y.wait(yv, ypend);
   #pragma unroll 1
-          for (int i = 0; uni(i < k); ++i) {
-            const int idx_next = (idx + 1 == M) ? 0 : idx + 1;
+          for (int i = 0; uni(i < ks); ++i) {
+            const int idx_next = (idx + 1 == MS) ? 0 : idx + 1;
             const auto part = lane_dot_p<P, T, E>(yv, q);
             T sv[E];
             SV::load(S + idx * SM::kVec, lane, sv);
             Y.issue(idx_next, yv, ypend);  // prefetch (harmless past the end: a valid slot)
             const T beta = rho_s[idx] * warp_sum_p<P, T, E>(part, rc);
             Y.wait(yv, ypend);
-            if (uni((valid >> idx) & 1u)) {  // lbfgs.h:189 skip
+            if (uni((valid >> i) & 1u)) {  // lbfgs.h:189 skip
               const T coef = alpha[i] - beta;
   #pragma unroll
               for (int j = 0; j < E; ++j) q[j] = q[j] + sv[j] * coef;
             }
             idx = idx_next;
+          }
+        }
+#pragma unroll
+        for (int j = R - 1; j >= 0; --j) {
+          if (uni(j < kr)) {
+            const auto part = lane_dot_p<P, T, E>(ry[j], q);
+            const T beta = rrho[j] * warp_sum_p<P, T, E>(part, rc);
+            if (uni((valid >> (k - 1 - j)) & 1u)) {  // lbfgs.h:189 skip
+              const T coef = ra[j] - beta;
+#pragma unroll
+              for (int e = 0; e < E; ++e) q[e] = q[e] + rs[j][e] * coef;
+            }
           }
         }
       }
@@ -453,7 +544,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         // along -search_direction = +g (SURVEY.md 7.2a): dginit = g.g >= 0.
 #pragma unroll
         for (int j = 0; j < E; ++j) q[j] = -g[j];
-        mem_count = 0;
+        mem_count = 0;  // (empties the register pairs as well)
         mem_pos = 0;
         valid = 0;
         const T gg = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(g, g), rc);  // :221 (rare path)
@@ -497,21 +588,45 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         // s.y > eps ||s|| ||y|| (:266), decided without the two square roots whenever a rigorous bound allows
         const bool curvature_ok = curvature_above_eps<T>(sy, ss, yy);
         if (uni(curvature_ok)) {
-          int slot;
+          // s.y is exactly the dot the reference recomputes per use; cache 1/(s.y)
+          const T rho_new = T(1) / sy;
+          if (uni(mem_count >= R)) {
+            // a pair enters the shared ring: the oldest register pair, or (R = 0) the new one; when the ring
+            // is full it replaces the oldest pair there, which leaves the history
+            int slot = mem_count - R;
+            if (slot == MS) {
+              slot = mem_pos;
+              mem_pos = (mem_pos + 1 == MS) ? 0 : mem_pos + 1;
+            }
+            if constexpr (R > 0) {
+              SV::store(S + slot * SM::kVec, lane, rs[R - 1]);
+              Y.store(slot, ry[R - 1]);
+            } else {
+              SV::store(S + slot * SM::kVec, lane, sd);
+              Y.store(slot, yd);
+            }
+            Y.fence_store();
+            __syncwarp();  // all lanes are done reading rho_s in this iteration's loops
+            if (lane == 0) rho_s[slot] = (R > 0) ? rrho[RA - 1] : rho_new;
+          }
+#pragma unroll
+          for (int j = R - 1; j > 0; --j) {  // register moves, newest pair into slot 0
+#pragma unroll
+            for (int e = 0; e < E; ++e) { rs[j][e] = rs[j - 1][e]; ry[j][e] = ry[j - 1][e]; }
+            rrho[j] = rrho[j - 1];
+          }
+          if constexpr (R > 0) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) { rs[0][e] = sd[e]; ry[0][e] = yd[e]; }
+            rrho[0] = rho_new;
+          }
+          const unsigned usable = (cabs(sy) < eps) ? 0u : 1u;
           if (mem_count < M) {
-            slot = mem_count;
+            valid |= usable << mem_count;
             mem_count++;
           } else {
-            slot = mem_pos;
-            mem_pos = (mem_pos + 1 == M) ? 0 : mem_pos + 1;
+            valid = (valid >> 1) | (usable << (M - 1));
           }
-          SV::store(S + slot * SM::kVec, lane, sd);
-          Y.store(slot, yd);
-          Y.fence_store();
-          // s.y is exactly the dot the reference recomputes per use; cache 1/(s.y)
-          __syncwarp();  // all lanes are done reading rho_s in this iteration's loops
-          if (lane == 0) rho_s[slot] = T(1) / sy;
-          valid = (cabs(sy) < eps) ? (valid & ~(1u << slot)) : (valid | (1u << slot));
         }
         if (yy > eps) {
           const T temp_scaling = sy / yy;
