@@ -21,6 +21,7 @@
 #include "cno_bfgs.cuh"
 #include "cno_descent.cuh"
 #include "cno_evaluate.cuh"
+#include "cno_launch.cuh"
 #include "cno_newton.cuh"
 #include "cno_newton_dmma.cuh"
 #include "cno_logistic.cuh"
@@ -31,7 +32,6 @@
 namespace {
 
 thread_local cudaError_t g_last_cuda = cudaSuccess;
-thread_local cno_launch_info_t g_last_info;
 
 #define CNO_CUDA(expr)                       \
   do {                                       \
@@ -71,13 +71,14 @@ struct HostArena {
 };
 HostArena g_host_arena;
 
-int device_sm_count(int* sms) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) { g_last_cuda = e; return CNO_ERR_NO_DEVICE; }
-  e = cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev);
-  if (e != cudaSuccess) { g_last_cuda = e; return CNO_ERR_NO_DEVICE; }
-  return CNO_OK;
+int default_policy(int dtype) { return dtype == CNO_F64 ? CNO_POLICY_DMMA_TREE : CNO_POLICY_WARP_TREE; }
+
+// problem->data holds a block of at least `elems` scalars per instance; blocks that TMA bulk copies read must also
+// be 16-byte aligned.
+template <class T>
+bool data_block_ok(const cno_problem_t* p, int64_t elems, bool tma_aligned) {
+  if (!p->data || p->data_stride < elems) return false;
+  return !tma_aligned || (((uintptr_t)p->data & 15) == 0 && ((size_t)p->data_stride * sizeof(T)) % 16 == 0);
 }
 
 struct LaunchArgs {
@@ -92,274 +93,112 @@ struct LaunchArgs {
   cno::ResumeArgs resume = cno::ResumeArgs{nullptr, 0, 0, 0};  // stepwise solves only
 };
 
-// One persistent launch of lbfgs_minimize_kernel<Fn, M[, kResume]>.
-template <class Fn, int M, bool kResume = false, class LS = cno::LsMoreThuente>
-int launch_lbfgs(const Fn& fn, const LaunchArgs& a) {
+// One persistent launch of a solve kernel(fn, x0, batch, stop, out, queue, extra...); the queue counter is the
+// first 8 bytes of the workspace.  A is LaunchArgs or LbfgsbArgs.
+template <class Plan, class Fn, class Kernel, class A, class... Extra>
+int launch_solve(Kernel kernel, const Fn& fn, const A& a, const Extra&... extra) {
   using T = typename Fn::Scalar;
-  using SM = typename cno::LbfgsPlan<Fn, M, kResume, LS>::SM;
-  auto kernel = cno::lbfgs_minimize_kernel<Fn, M, kResume, LS>;
-  const size_t smem = SM::kWarpBytes * SM::kWarps;
-  CNO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int sms = 0;
-  int rc = device_sm_count(&sms);
-  if (rc) return rc;
-  // never launch more warps than instances
-  long long ctas = (a.batch + SM::kWarps - 1) / SM::kWarps;
-  const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
   unsigned long long* queue = static_cast<unsigned long long*>(a.workspace);
-  CNO_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), a.stream));
-  const cno::StopParams<T> stop = cno::make_stop<T>(*a.stop);
-  const cno::BatchOut<T> out = cno::make_out<T>(*a.out);
-  kernel<<<grid, SM::kThreads, smem, a.stream>>>(fn, static_cast<const T*>(a.x0), a.batch,
-                                                 stop, out, queue, a.resume);
-  CNO_CUDA(cudaGetLastError());
-  if (a.info) {
-    a.info->kernel_launches += 1;
-    a.info->grid = grid;
-    a.info->block = SM::kThreads;
-    a.info->warps_per_cta = SM::kWarps;
-    a.info->dynamic_smem = (int64_t)smem;
-  }
-  return CNO_OK;
+  return cno::launch_persistent<Plan>(kernel, a.batch, queue, a.stream, a.info, g_last_cuda, fn,
+                                      static_cast<const T*>(a.x0), a.batch, cno::make_stop<T>(*a.stop),
+                                      cno::make_out<T>(*a.out), queue, extra...);
 }
 
-// One persistent launch of bfgs_minimize_kernel<Fn> (D <= 32: inverse Hessian in registers) or
-// bfgs_smem_minimize_kernel<Fn> (D > 32: in shared memory).
-template <class Fn, class LS, bool kBig = (Fn::Dim > 32)>
-struct BfgsKernelOf {
-  using SM = cno::BfgsSmem<typename Fn::Scalar, Fn::Dim>;
-  static auto kernel() { return cno::bfgs_minimize_kernel<Fn, LS>; }
-};
-template <class Fn, class LS>
-struct BfgsKernelOf<Fn, LS, true> {
-  using SM = cno::BfgsBigSmem<typename Fn::Scalar, Fn::Dim>;
-  static auto kernel() { return cno::bfgs_smem_minimize_kernel<Fn, LS>; }
-};
+template <class Fn, int M = CNO_LBFGS_M, bool kResume = false, class LS = cno::LsMoreThuente>
+int lbfgs(const Fn& fn, const LaunchArgs& a) {
+  return launch_solve<typename cno::LbfgsPlan<Fn, M, kResume, LS>::SM>(cno::lbfgs_minimize_kernel<Fn, M, kResume, LS>,
+                                                                      fn, a, a.resume);
+}
 template <class Fn, class LS = cno::LsMoreThuente>
-int launch_bfgs(const Fn& fn, const LaunchArgs& a) {
-  using T = typename Fn::Scalar;
-  using SM = typename BfgsKernelOf<Fn, LS>::SM;
-  auto kernel = BfgsKernelOf<Fn, LS>::kernel();
-  const size_t smem = SM::kWarpBytes * SM::kWarps;
-  CNO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int sms = 0;
-  int rc = device_sm_count(&sms);
-  if (rc) return rc;
-  long long ctas = (a.batch + SM::kWarps - 1) / SM::kWarps;
-  const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
-  unsigned long long* queue = static_cast<unsigned long long*>(a.workspace);
-  CNO_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), a.stream));
-  const cno::StopParams<T> stop = cno::make_stop<T>(*a.stop);
-  const cno::BatchOut<T> out = cno::make_out<T>(*a.out);
-  kernel<<<grid, SM::kWarps * 32, smem, a.stream>>>(fn, static_cast<const T*>(a.x0), a.batch,
-                                                    stop, out, queue);
-  CNO_CUDA(cudaGetLastError());
-  if (a.info) {
-    a.info->kernel_launches += 1;
-    a.info->grid = grid;
-    a.info->block = SM::kWarps * 32;
-    a.info->warps_per_cta = SM::kWarps;
-    a.info->dynamic_smem = (int64_t)smem;
-  }
-  return CNO_OK;
+int bfgs(const Fn& fn, const LaunchArgs& a) {
+  return launch_solve<typename cno::BfgsPlan<Fn, LS>::SM>(cno::BfgsPlan<Fn, LS>::kernel(), fn, a);
 }
-
-// One persistent launch of descent_minimize_kernel<Fn, kConjugate>
-// (GradientDescent / ConjugatedGradientDescent).
+// GradientDescent (kConjugate = false) / ConjugatedGradientDescent
 template <class Fn, bool kConjugate, class LS = cno::LsMoreThuente>
-int launch_descent(const Fn& fn, const LaunchArgs& a) {
-  using T = typename Fn::Scalar;
-  using SM = cno::DescentSmem<T>;
-  auto kernel = cno::descent_minimize_kernel<Fn, kConjugate, LS>;
-  const size_t smem = SM::kWarpBytes * SM::kWarps;
-  int sms = 0;
-  int rc = device_sm_count(&sms);
-  if (rc) return rc;
-  long long ctas = (a.batch + SM::kWarps - 1) / SM::kWarps;
-  const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
-  unsigned long long* queue = static_cast<unsigned long long*>(a.workspace);
-  CNO_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), a.stream));
-  const cno::StopParams<T> stop = cno::make_stop<T>(*a.stop);
-  const cno::BatchOut<T> out = cno::make_out<T>(*a.out);
-  kernel<<<grid, SM::kWarps * 32, smem, a.stream>>>(fn, static_cast<const T*>(a.x0), a.batch,
-                                                    stop, out, queue);
-  CNO_CUDA(cudaGetLastError());
-  if (a.info) {
-    a.info->kernel_launches += 1;
-    a.info->grid = grid;
-    a.info->block = SM::kWarps * 32;
-    a.info->warps_per_cta = SM::kWarps;
-    a.info->dynamic_smem = (int64_t)smem;
-  }
-  return CNO_OK;
+int descent(const Fn& fn, const LaunchArgs& a) {
+  return launch_solve<cno::DescentSmem<typename Fn::Scalar>>(cno::descent_minimize_kernel<Fn, kConjugate, LS>, fn, a);
 }
-
-// One persistent launch of newton_minimize_kernel<Fn>.
 template <class Fn>
-int launch_newton(const Fn& fn, const LaunchArgs& a) {
-  using T = typename Fn::Scalar;
-  using SM = cno::NewtonSmem<T, Fn::Dim>;
+int newton(const Fn& fn, const LaunchArgs& a) {
   if (a.stop->condition_hessian > 0) return CNO_ERR_UNSUPPORTED;  // see cno_newton.cuh
-  auto kernel = cno::newton_minimize_kernel<Fn>;
-  const size_t smem = SM::kWarpBytes * SM::kWarps;
-  CNO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int sms = 0;
-  int rc = device_sm_count(&sms);
-  if (rc) return rc;
-  long long ctas = (a.batch + SM::kWarps - 1) / SM::kWarps;
-  const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
-  unsigned long long* queue = static_cast<unsigned long long*>(a.workspace);
-  CNO_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), a.stream));
-  const cno::StopParams<T> stop = cno::make_stop<T>(*a.stop);
-  const cno::BatchOut<T> out = cno::make_out<T>(*a.out);
-  kernel<<<grid, SM::kWarps * 32, smem, a.stream>>>(fn, static_cast<const T*>(a.x0), a.batch,
-                                                    stop, out, queue);
-  CNO_CUDA(cudaGetLastError());
-  if (a.info) {
-    a.info->kernel_launches += 1;
-    a.info->grid = grid;
-    a.info->block = SM::kWarps * 32;
-    a.info->warps_per_cta = SM::kWarps;
-    a.info->dynamic_smem = (int64_t)smem;
-  }
-  return CNO_OK;
+  return launch_solve<cno::NewtonSmem<typename Fn::Scalar, Fn::Dim>>(cno::newton_minimize_kernel<Fn>, fn, a);
 }
 
 template <class T, int D>
 int newton_dense_quadratic(const LaunchArgs& a) {
   const cno_problem_t* p = a.problem;
-  if (!p->data || p->data_stride < (int64_t)D * D + D) return CNO_ERR_INVALID_ARGUMENT;
-  if (((uintptr_t)p->data & 15) || ((size_t)p->data_stride * sizeof(T)) % 16)
-    return CNO_ERR_INVALID_ARGUMENT;  // TMA bulk copies need 16-byte aligned blocks
-  return launch_newton<cno::DenseQuadraticFn<T, D>>(
-      cno::DenseQuadraticFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
+  if (!data_block_ok<T>(p, (int64_t)D * D + D, true)) return CNO_ERR_INVALID_ARGUMENT;
+  return newton(cno::DenseQuadraticFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
 }
 // CNO_POLICY_DMMA_LU: d = 64 fp64 dense quadratic, blocked LU with the trailing update on the FP64 tensor core
 // (csrc/cno_newton_dmma.cuh).
-int launch_newton_dmma(const cno::DenseQuadraticDmmaFn& fn, const LaunchArgs& a) {
-  using Fn = cno::DenseQuadraticDmmaFn;
-  using SM = cno::NewtonDmmaSmem;
-  auto kernel = cno::newton_dmma_minimize_kernel<Fn>;
-  const size_t smem = SM::kBytes;
-  CNO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int sms = 0;
-  int rc = device_sm_count(&sms);
-  if (rc) return rc;
-  long long ctas = (a.batch + SM::kWarps - 1) / SM::kWarps;
-  const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
-  unsigned long long* queue = static_cast<unsigned long long*>(a.workspace);
-  CNO_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), a.stream));
-  const cno::StopParams<double> stop = cno::make_stop<double>(*a.stop);
-  const cno::BatchOut<double> out = cno::make_out<double>(*a.out);
-  kernel<<<grid, SM::kWarps * 32, smem, a.stream>>>(fn, static_cast<const double*>(a.x0), a.batch, stop, out, queue);
-  CNO_CUDA(cudaGetLastError());
-  if (a.info) {
-    a.info->kernel_launches += 1;
-    a.info->grid = grid;
-    a.info->block = SM::kWarps * 32;
-    a.info->warps_per_cta = SM::kWarps;
-    a.info->dynamic_smem = (int64_t)smem;
-  }
-  return CNO_OK;
-}
 int newton_dense_quadratic_dmma(const LaunchArgs& a) {
+  using Fn = cno::DenseQuadraticDmmaFn;
   const cno_problem_t* p = a.problem;
-  if (!p->data || p->data_stride < (int64_t)64 * 64 + 64) return CNO_ERR_INVALID_ARGUMENT;
-  if (((uintptr_t)p->data & 15) || ((size_t)p->data_stride * sizeof(double)) % 16) return CNO_ERR_INVALID_ARGUMENT;
+  if (!data_block_ok<double>(p, (int64_t)64 * 64 + 64, true)) return CNO_ERR_INVALID_ARGUMENT;
   if (a.stop->condition_hessian > 0) return CNO_ERR_UNSUPPORTED;  // see cno_newton.cuh
-  cno::DenseQuadraticDmmaFn fn;
+  Fn fn;
   fn.data = static_cast<const double*>(p->data);
   fn.stride = (long long)p->data_stride;
-  return launch_newton_dmma(fn, a);
+  return launch_solve<cno::NewtonDmmaSmem>(cno::newton_dmma_minimize_kernel<Fn>, fn, a);
 }
 template <class T, int D>
-int newton_rosenbrock(const LaunchArgs& a) {
-  return launch_newton<cno::RosenbrockFullFn<T, D>>(cno::RosenbrockFullFn<T, D>{}, a);
-}
+int newton_rosenbrock(const LaunchArgs& a) { return newton(cno::RosenbrockFullFn<T, D>{}, a); }
 
 template <class T, int D>
-int bfgs_rosenbrock(const LaunchArgs& a) {
-  return launch_bfgs<cno::RosenbrockFn<T, D>>(cno::RosenbrockFn<T, D>{}, a);
-}
+int bfgs_rosenbrock(const LaunchArgs& a) { return bfgs(cno::RosenbrockFn<T, D>{}, a); }
 template <class T, int D>
-int bfgs_half_sq_norm(const LaunchArgs& a) {
-  return launch_bfgs<cno::HalfSquaredNormFn<T, D>>(cno::HalfSquaredNormFn<T, D>{}, a);
-}
+int bfgs_half_sq_norm(const LaunchArgs& a) { return bfgs(cno::HalfSquaredNormFn<T, D>{}, a); }
 template <class T>
-int bfgs_diag_quadratic(const LaunchArgs& a) {
-  return launch_bfgs<cno::DiagQuadraticFn<T>>(cno::DiagQuadraticFn<T>{}, a);
-}
+int bfgs_diag_quadratic(const LaunchArgs& a) { return bfgs(cno::DiagQuadraticFn<T>{}, a); }
 
 // LineSearch = HagerZhang variants (CNO_*_HAGER_ZHANG)
 template <class T, int D>
 int lbfgs_rosenbrock_hz(const LaunchArgs& a) {
-  return launch_lbfgs<cno::RosenbrockFn<T, D>, CNO_LBFGS_M, false, cno::LsHagerZhang>(cno::RosenbrockFn<T, D>{}, a);
+  return lbfgs<cno::RosenbrockFn<T, D>, CNO_LBFGS_M, false, cno::LsHagerZhang>(cno::RosenbrockFn<T, D>{}, a);
 }
 template <class T, int D>
-int bfgs_rosenbrock_hz(const LaunchArgs& a) {
-  return launch_bfgs<cno::RosenbrockFn<T, D>, cno::LsHagerZhang>(cno::RosenbrockFn<T, D>{}, a);
-}
+int bfgs_rosenbrock_hz(const LaunchArgs& a) { return bfgs<cno::RosenbrockFn<T, D>, cno::LsHagerZhang>({}, a); }
 template <class T, int D>
-int gd_rosenbrock_hz(const LaunchArgs& a) {
-  return launch_descent<cno::RosenbrockFn<T, D>, false, cno::LsHagerZhang>(cno::RosenbrockFn<T, D>{}, a);
-}
+int gd_rosenbrock_hz(const LaunchArgs& a) { return descent<cno::RosenbrockFn<T, D>, false, cno::LsHagerZhang>({}, a); }
 
 template <class T, int D, bool kConjugate>
-int descent_rosenbrock(const LaunchArgs& a) {
-  return launch_descent<cno::RosenbrockFn<T, D>, kConjugate>(cno::RosenbrockFn<T, D>{}, a);
-}
+int descent_rosenbrock(const LaunchArgs& a) { return descent<cno::RosenbrockFn<T, D>, kConjugate>({}, a); }
 template <class T, bool kConjugate>
-int descent_diag_quadratic(const LaunchArgs& a) {
-  return launch_descent<cno::DiagQuadraticFn<T>, kConjugate>(cno::DiagQuadraticFn<T>{}, a);
-}
+int descent_diag_quadratic(const LaunchArgs& a) { return descent<cno::DiagQuadraticFn<T>, kConjugate>({}, a); }
 
 template <class T, int D>
-int lbfgs_rosenbrock(const LaunchArgs& a) {
-  return launch_lbfgs<cno::RosenbrockFn<T, D>, CNO_LBFGS_M>(cno::RosenbrockFn<T, D>{}, a);
-}
+int lbfgs_rosenbrock(const LaunchArgs& a) { return lbfgs(cno::RosenbrockFn<T, D>{}, a); }
 // Lbfgs<F, m> for m other than the default (lbfgs.h:40-41)
 template <class T, int D, int M>
-int lbfgs_rosenbrock_m(const LaunchArgs& a) {
-  return launch_lbfgs<cno::RosenbrockFn<T, D>, M>(cno::RosenbrockFn<T, D>{}, a);
-}
+int lbfgs_rosenbrock_m(const LaunchArgs& a) { return lbfgs<cno::RosenbrockFn<T, D>, M>({}, a); }
 // "parity mode": Eigen-SSE2-model reduction order (CNO_POLICY_EIGEN_SSE2), d = 128 fp64
 int lbfgs_rosenbrock_d128_eigen(const LaunchArgs& a) {
-  using Fn = cno::RosenbrockFn<double, 128, cno::PolicyEigenSSE2>;
-  return launch_lbfgs<Fn, CNO_LBFGS_M>(Fn{}, a);
+  return lbfgs(cno::RosenbrockFn<double, 128, cno::PolicyEigenSSE2>{}, a);
 }
 // Lbfgs on a Second-mode function: diagonal-preconditioner branch (lbfgs.h:116-139)
 template <class T, int D>
 int lbfgs_rosenbrock_second(const LaunchArgs& a) {
-  using Fn = cno::SecondMode<cno::RosenbrockFn<T, D>>;
   if (a.stop->condition_hessian > 0) return CNO_ERR_UNSUPPORTED;  // not computed (cno_newton.cuh)
-  return launch_lbfgs<Fn, CNO_LBFGS_M>(Fn{}, a);
+  return lbfgs(cno::SecondMode<cno::RosenbrockFn<T, D>>{}, a);
 }
 // First-mode dense quadratic ([A | b] read from global memory per evaluation)
 template <class T, int D>
 int lbfgs_dense_quadratic(const LaunchArgs& a) {
   const cno_problem_t* p = a.problem;
-  if (!p->data || p->data_stride < (int64_t)D * D + D) return CNO_ERR_INVALID_ARGUMENT;
-  using Fn = cno::DenseQuadraticGlobalFn<T, D>;
-  return launch_lbfgs<Fn, CNO_LBFGS_M>(Fn{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
+  if (!data_block_ok<T>(p, (int64_t)D * D + D, false)) return CNO_ERR_INVALID_ARGUMENT;
+  return lbfgs(cno::DenseQuadraticGlobalFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
 }
 template <class T, int D>
-int lbfgs_half_sq_norm(const LaunchArgs& a) {
-  return launch_lbfgs<cno::HalfSquaredNormFn<T, D>, CNO_LBFGS_M>(cno::HalfSquaredNormFn<T, D>{}, a);
-}
+int lbfgs_half_sq_norm(const LaunchArgs& a) { return lbfgs(cno::HalfSquaredNormFn<T, D>{}, a); }
 template <class T>
-int lbfgs_diag_quadratic(const LaunchArgs& a) {
-  return launch_lbfgs<cno::DiagQuadraticFn<T>, CNO_LBFGS_M>(cno::DiagQuadraticFn<T>{}, a);
-}
+int lbfgs_diag_quadratic(const LaunchArgs& a) { return lbfgs(cno::DiagQuadraticFn<T>{}, a); }
 
 // Stepwise variants (cno_minimize_steps): same kernel with park / un-park code.
 template <class T, int D>
-int lbfgs_rosenbrock_steps(const LaunchArgs& a) {
-  return launch_lbfgs<cno::RosenbrockFn<T, D>, CNO_LBFGS_M, true>(cno::RosenbrockFn<T, D>{}, a);
-}
+int lbfgs_rosenbrock_steps(const LaunchArgs& a) { return lbfgs<cno::RosenbrockFn<T, D>, CNO_LBFGS_M, true>({}, a); }
 template <class Fn>
-int lbfgs_steps_stateless(const LaunchArgs& a) {  // functors without parameters
-  return launch_lbfgs<Fn, CNO_LBFGS_M, true>(Fn{}, a);
-}
+int lbfgs_steps_stateless(const LaunchArgs& a) { return lbfgs<Fn, CNO_LBFGS_M, true>({}, a); }  // functors without parameters
 template <class T, int D>
 size_t lbfgs_state_stride() {
   return cno::ResumeLayout<T, cno::Shape<D>::E, CNO_LBFGS_M>::kBytes;
@@ -369,10 +208,8 @@ template <class T, int D, int N>
 int lbfgs_logistic(const LaunchArgs& a) {
   const cno_problem_t* p = a.problem;
   using Fn = cno::LogisticFn<T, D, N>;
-  if (p->n != N || !p->data || p->data_stride < (int64_t)Fn::kBlockElems) return CNO_ERR_INVALID_ARGUMENT;
-  if (((uintptr_t)p->data & 15) || ((size_t)p->data_stride * sizeof(T)) % 16)
-    return CNO_ERR_INVALID_ARGUMENT;  // TMA bulk copies need 16-byte aligned blocks
-  return launch_lbfgs<Fn, CNO_LBFGS_M>(Fn{static_cast<const T*>(p->data), (long long)p->data_stride, (T)p->param}, a);
+  if (p->n != N || !data_block_ok<T>(p, Fn::kBlockElems, true)) return CNO_ERR_INVALID_ARGUMENT;
+  return lbfgs(Fn{static_cast<const T*>(p->data), (long long)p->data_stride, (T)p->param}, a);
 }
 
 // ---- Progress::condition_hessian on request (csrc/cno_newton.cuh: condition_hessian_kernel) ----
@@ -387,26 +224,16 @@ struct CondArgs {
 template <class Fn>
 int launch_condition(const Fn& fn, const CondArgs& a) {
   using T = typename Fn::Scalar;
-  using CS = cno::ConditionSmem<T, Fn::Dim>;
-  auto kernel = cno::condition_hessian_kernel<Fn>;
-  const size_t smem = CS::kWarpBytes * CS::kWarps;
-  CNO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int sms = 0;
-  int rc = device_sm_count(&sms);
-  if (rc) return rc;
-  long long ctas = (a.batch + CS::kWarps - 1) / CS::kWarps;
-  const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
   unsigned long long* queue = static_cast<unsigned long long*>(a.workspace);
-  CNO_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), a.stream));
-  kernel<<<grid, CS::kWarps * 32, smem, a.stream>>>(fn, static_cast<const T*>(a.x), a.batch, static_cast<T*>(a.out), queue);
-  CNO_CUDA(cudaGetLastError());
-  return CNO_OK;
+  return cno::launch_persistent<cno::ConditionSmem<T, Fn::Dim>>(cno::condition_hessian_kernel<Fn>, a.batch, queue,
+                                                                a.stream, nullptr, g_last_cuda, fn,
+                                                                static_cast<const T*>(a.x), a.batch,
+                                                                static_cast<T*>(a.out), queue);
 }
 template <class T, int D>
 int condition_dense_quadratic(const CondArgs& a) {
   const cno_problem_t* p = a.problem;
-  if (!p->data || p->data_stride < (int64_t)D * D + D) return CNO_ERR_INVALID_ARGUMENT;
-  if (((uintptr_t)p->data & 15) || ((size_t)p->data_stride * sizeof(T)) % 16) return CNO_ERR_INVALID_ARGUMENT;
+  if (!data_block_ok<T>(p, (int64_t)D * D + D, true)) return CNO_ERR_INVALID_ARGUMENT;
   return launch_condition(cno::DenseQuadraticFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
 }
 template <class T, int D>
@@ -528,49 +355,28 @@ struct LbfgsbArgs {
   cno_launch_info_t* info;
 };
 template <class Fn, int M = 5>
-int launch_lbfgsb(const Fn& fn, const LbfgsbArgs& a) {
+int lbfgsb(const Fn& fn, const LbfgsbArgs& a) {
   using T = typename Fn::Scalar;
-  using SM = cno::LbfgsbSmem<T, Fn::Dim, M>;
-  auto kernel = cno::lbfgsb_minimize_kernel<Fn, M>;
-  const size_t smem = SM::kWarpBytes * SM::kWarps;
-  CNO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int sms = 0;
-  int rc = device_sm_count(&sms);
-  if (rc) return rc;
-  long long ctas = (a.batch + SM::kWarps - 1) / SM::kWarps;
-  const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
-  unsigned long long* queue = static_cast<unsigned long long*>(a.workspace);
-  CNO_CUDA(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), a.stream));
   const cno::BoundsArgs<T> bd{a.bounds ? static_cast<const T*>(a.bounds->lower) : nullptr,
                               a.bounds ? static_cast<const T*>(a.bounds->upper) : nullptr,
                               a.bounds ? (long long)a.bounds->stride : 0};
-  kernel<<<grid, SM::kWarps * 32, smem, a.stream>>>(fn, static_cast<const T*>(a.x0), a.batch, cno::make_stop<T>(*a.stop),
-                                                    cno::make_out<T>(*a.out), queue, bd);
-  CNO_CUDA(cudaGetLastError());
-  if (a.info) {
-    a.info->kernel_launches += 1;
-    a.info->grid = grid;
-    a.info->block = SM::kWarps * 32;
-    a.info->warps_per_cta = SM::kWarps;
-    a.info->dynamic_smem = (int64_t)smem;
-  }
-  return CNO_OK;
+  return launch_solve<cno::LbfgsbSmem<T, Fn::Dim, M>>(cno::lbfgsb_minimize_kernel<Fn, M>, fn, a, bd);
 }
 template <class T, int D>
-int lbfgsb_rosenbrock(const LbfgsbArgs& a) { return launch_lbfgsb(cno::RosenbrockFn<T, D>{}, a); }
+int lbfgsb_rosenbrock(const LbfgsbArgs& a) { return lbfgsb(cno::RosenbrockFn<T, D>{}, a); }
 template <class T, int D>
-int lbfgsb_half_sq_norm(const LbfgsbArgs& a) { return launch_lbfgsb(cno::HalfSquaredNormFn<T, D>{}, a); }
+int lbfgsb_half_sq_norm(const LbfgsbArgs& a) { return lbfgsb(cno::HalfSquaredNormFn<T, D>{}, a); }
 template <class T>
-int lbfgsb_diag_quadratic(const LbfgsbArgs& a) { return launch_lbfgsb(cno::DiagQuadraticFn<T>{}, a); }
+int lbfgsb_diag_quadratic(const LbfgsbArgs& a) { return lbfgsb(cno::DiagQuadraticFn<T>{}, a); }
 template <class T, int D>
 int lbfgsb_dense_quadratic(const LbfgsbArgs& a) {
   const cno_problem_t* p = a.problem;
-  if (!p->data || p->data_stride < (int64_t)D * D + D) return CNO_ERR_INVALID_ARGUMENT;
-  return launch_lbfgsb(cno::DenseQuadraticGlobalFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
+  if (!data_block_ok<T>(p, (int64_t)D * D + D, false)) return CNO_ERR_INVALID_ARGUMENT;
+  return lbfgsb(cno::DenseQuadraticGlobalFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
 }
 // Lbfgsb<F, m> for m other than the default 5 (lbfgsb.h:44-45)
 template <class T, int D, int M>
-int lbfgsb_rosenbrock_m(const LbfgsbArgs& a) { return launch_lbfgsb<cno::RosenbrockFn<T, D>, M>(cno::RosenbrockFn<T, D>{}, a); }
+int lbfgsb_rosenbrock_m(const LbfgsbArgs& a) { return lbfgsb<cno::RosenbrockFn<T, D>, M>({}, a); }
 struct LbfgsbEntry { int family, dtype, d; int (*fn)(const LbfgsbArgs&); int m = 5; };
 const LbfgsbEntry kLbfgsbTable[] = {
     {CNO_FN_ROSENBROCK, CNO_F64, 8, lbfgsb_rosenbrock_m<double, 8, 10>, 10},
@@ -589,9 +395,7 @@ const LbfgsbEntry kLbfgsbTable[] = {
     {CNO_FN_DENSE_QUADRATIC, CNO_F64, 64, lbfgsb_dense_quadratic<double, 64>},
 };
 const LbfgsbEntry* lbfgsb_find(const cno_problem_t* p) {
-  if (!p) return nullptr;
-  const int dflt = (p->dtype == CNO_F64) ? CNO_POLICY_DMMA_TREE : CNO_POLICY_WARP_TREE;
-  if (p->policy != dflt) return nullptr;
+  if (!p || p->policy != default_policy(p->dtype)) return nullptr;
   const int m = p->lbfgs_m > 0 ? p->lbfgs_m : 5;  // cno_problem_t::lbfgs_m: pairs kept (0 = the reference's default, 5)
   for (const LbfgsbEntry& e : kLbfgsbTable)
     if (e.family == p->family && e.dtype == p->dtype && e.d == p->d && e.m == m) return &e;
@@ -614,7 +418,7 @@ int eval_half_sq_norm(const cno_problem_t*, int64_t b, const void* x, void* f, v
 }
 template <class T, int D>
 int eval_dense_quadratic(const cno_problem_t* p, int64_t b, const void* x, void* f, void* g, void* s) {
-  if (!p->data || p->data_stride < (int64_t)D * D + D) return CNO_ERR_INVALID_ARGUMENT;
+  if (!data_block_ok<T>(p, (int64_t)D * D + D, false)) return CNO_ERR_INVALID_ARGUMENT;
   return cno::launch_evaluate(cno::DenseQuadraticGlobalFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride},
                               b, x, f, g, s);
 }
@@ -636,7 +440,7 @@ const EvalEntry kEvalTable[] = {
 };
 
 const Entry* find_entry(int solver, const cno_problem_t* p) {
-  const int dflt = (p->dtype == CNO_F64) ? CNO_POLICY_DMMA_TREE : CNO_POLICY_WARP_TREE;
+  const int dflt = default_policy(p->dtype);
   const bool is_lbfgs = (solver == CNO_LBFGS || solver == CNO_LBFGS_HAGER_ZHANG);
   const int m = (is_lbfgs && p->lbfgs_m > 0) ? p->lbfgs_m : CNO_LBFGS_M;
   for (const Entry& e : kTable)
@@ -786,7 +590,7 @@ struct AlCudaBackend {
     inner_out.nfev = const_cast<uint32_t*>(a.inner_nfev);
     cno_launch_info_t inner_info{};
     const LaunchArgs la{A.objective, A.batch, a.x, &stop, &inner_out, queue, s, &inner_info};
-    return launch_lbfgs<cno::AugLagFn<Obj>, CNO_LBFGS_M>(composite, la);
+    return lbfgs(composite, la);
   }
   int outer_step(int* remaining) {
     CNO_CUDA(cudaMemsetAsync(a.remaining, 0, sizeof(int), s));
@@ -828,7 +632,7 @@ int al_half_sq_norm(const AlArgs& a) { return al_run(cno::HalfSquaredNormFn<T, D
 template <class T, int D>
 int al_dense_quadratic(const AlArgs& a) {  // the batched "QP with affine / ball constraints"
   const cno_problem_t* p = a.objective;
-  if (!p->data || p->data_stride < (int64_t)D * D + D) return CNO_ERR_INVALID_ARGUMENT;
+  if (!data_block_ok<T>(p, (int64_t)D * D + D, false)) return CNO_ERR_INVALID_ARGUMENT;
   return al_run(cno::DenseQuadraticGlobalFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
 }
 
@@ -849,8 +653,7 @@ const AlEntry kAlTable[] = {
 };
 
 const AlEntry* al_find(const cno_problem_t* p) {
-  const int dflt = (p->dtype == CNO_F64) ? CNO_POLICY_DMMA_TREE : CNO_POLICY_WARP_TREE;
-  if (p->policy != dflt || p->mode == 2) return nullptr;
+  if (p->policy != default_policy(p->dtype) || p->mode == 2) return nullptr;
   for (const AlEntry& e : kAlTable)
     if (e.family == p->family && e.dtype == p->dtype && e.d == p->d) return &e;
   return nullptr;
@@ -871,6 +674,25 @@ bool have_device() {
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess) { g_last_cuda = e; (void)cudaGetLastError(); return false; }
   return n > 0;
+}
+
+// NULL stop = the preset `dflt` writes into *local; a `past` beyond the kernels' CNO_MAX_PAST ring is rejected.
+int resolve_stop(const cno_stop_t*& stop, cno_stop_t* local, void (*dflt)(cno_stop_t*)) {
+  if (!stop) {
+    dflt(local);
+    stop = local;
+  }
+  return (stop->past > CNO_MAX_PAST || stop->past < 0) ? CNO_ERR_INVALID_ARGUMENT : CNO_OK;
+}
+
+// the queue counter: 8-byte aligned, kWorkspaceBytes at least
+bool queue_workspace_ok(const void* workspace, size_t bytes) {
+  return workspace && bytes >= kWorkspaceBytes && !((uintptr_t)workspace & 7);
+}
+
+// the kernels load and store x and the gradient as 16-byte vectors
+bool io_aligned(const void* x0, const cno_batch_out_t* out) {
+  return !(((uintptr_t)x0 & 15) || ((uintptr_t)out->x & 15) || ((uintptr_t)out->gradient & 15));
 }
 
 }  // namespace
@@ -945,38 +767,19 @@ int cno_minimize(int solver, const cno_problem_t* problem, int64_t batch, const 
     return have_device() ? CNO_OK : CNO_ERR_NO_DEVICE;
   }
   if (!x0) return CNO_ERR_INVALID_ARGUMENT;
-  if (!workspace || workspace_bytes < kWorkspaceBytes || ((uintptr_t)workspace & 7))
-    return CNO_ERR_WORKSPACE;
-  if (((uintptr_t)x0 & 15) || ((uintptr_t)out->x & 15) || ((uintptr_t)out->gradient & 15))
-    return CNO_ERR_INVALID_ARGUMENT;
-  cno_stop_t dflt;
-  if (!stop) {
-    cno_default_stop(&dflt);
-    stop = &dflt;
-  }
-  if (stop->past > CNO_MAX_PAST || stop->past < 0) return CNO_ERR_INVALID_ARGUMENT;
+  if (!queue_workspace_ok(workspace, workspace_bytes)) return CNO_ERR_WORKSPACE;
+  if (!io_aligned(x0, out)) return CNO_ERR_INVALID_ARGUMENT;
+  cno_stop_t local;
+  if ((rc = resolve_stop(stop, &local, cno_default_stop))) return rc;
   if (!have_device()) return CNO_ERR_NO_DEVICE;
   if (info) memset(info, 0, sizeof(*info));
-  if (batch == 0) return CNO_OK;
 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  EventOwner e0, e1;
-  if (info) {
-    CNO_CUDA(e0.create());
-    CNO_CUDA(e1.create());
-    CNO_CUDA(cudaEventRecord(e0.e, s));
-  }
+  cno::LaunchTimer timer(s, info);
+  if ((rc = timer.start(g_last_cuda))) return rc;
   const LaunchArgs a{problem, (long long)batch, x0, stop, out, workspace, s, info};
-  rc = find_entry(solver, problem)->fn(a);
-  if (rc) return rc;
-  if (info) {
-    CNO_CUDA(cudaEventRecord(e1.e, s));
-    CNO_CUDA(cudaEventSynchronize(e1.e));
-    CNO_CUDA(cudaEventElapsedTime(&info->kernel_ms, e0.e, e1.e));
-    info->total_ms = info->kernel_ms;
-    g_last_info = *info;
-  }
-  return CNO_OK;
+  if ((rc = find_entry(solver, problem)->fn(a))) return rc;
+  return timer.stop(g_last_cuda);
 }
 
 int cno_state_bytes(int solver, const cno_problem_t* problem, int64_t batch, size_t* bytes) {
@@ -1006,32 +809,19 @@ int cno_minimize_steps(int solver, const cno_problem_t* problem, int64_t batch, 
   if (!x0 && first_call) return CNO_ERR_INVALID_ARGUMENT;
   const size_t stride = e->state_stride();
   if (!state || state_bytes < (size_t)batch * stride || ((uintptr_t)state & 15)) return CNO_ERR_WORKSPACE;
-  if (!workspace || workspace_bytes < kWorkspaceBytes || ((uintptr_t)workspace & 7)) return CNO_ERR_WORKSPACE;
-  if (((uintptr_t)x0 & 15) || ((uintptr_t)out->x & 15) || ((uintptr_t)out->gradient & 15))
-    return CNO_ERR_INVALID_ARGUMENT;
-  cno_stop_t dflt;
-  if (!stop) { cno_default_stop(&dflt); stop = &dflt; }
-  if (stop->past > CNO_MAX_PAST || stop->past < 0) return CNO_ERR_INVALID_ARGUMENT;
+  if (!queue_workspace_ok(workspace, workspace_bytes)) return CNO_ERR_WORKSPACE;
+  if (!io_aligned(x0, out)) return CNO_ERR_INVALID_ARGUMENT;
+  cno_stop_t local;
+  if ((rc = resolve_stop(stop, &local, cno_default_stop))) return rc;
   if (!have_device()) return CNO_ERR_NO_DEVICE;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  EventOwner e0, e1;
-  if (info) {
-    CNO_CUDA(e0.create());
-    CNO_CUDA(e1.create());
-    CNO_CUDA(cudaEventRecord(e0.e, s));
-  }
+  cno::LaunchTimer timer(s, info);
+  if ((rc = timer.start(g_last_cuda))) return rc;
   LaunchArgs a{problem, (long long)batch, x0, stop, out, workspace, s, info};
   a.resume = cno::ResumeArgs{static_cast<unsigned char*>(state), (long long)stride, max_iterations,
                              first_call ? 1 : 0};
-  rc = e->steps_fn(a);
-  if (rc) return rc;
-  if (info) {
-    CNO_CUDA(cudaEventRecord(e1.e, s));
-    CNO_CUDA(cudaEventSynchronize(e1.e));
-    CNO_CUDA(cudaEventElapsedTime(&info->kernel_ms, e0.e, e1.e));
-    info->total_ms = info->kernel_ms;
-  }
-  return CNO_OK;
+  if ((rc = e->steps_fn(a))) return rc;
+  return timer.stop(g_last_cuda);
 }
 
 int cno_minimize_host(int solver, const cno_problem_t* problem, int64_t batch, const void* x0,
@@ -1044,9 +834,8 @@ int cno_minimize_host(int solver, const cno_problem_t* problem, int64_t batch, c
   cno_launch_info_t local;
   memset(&local, 0, sizeof(local));
   if (batch == 0) { if (info) *info = local; return CNO_OK; }
-  cno_stop_t dflt;
-  if (!stop) { cno_default_stop(&dflt); stop = &dflt; }
-  if (stop->past > CNO_MAX_PAST || stop->past < 0) return CNO_ERR_INVALID_ARGUMENT;
+  cno_stop_t local_stop;
+  if ((rc = resolve_stop(stop, &local_stop, cno_default_stop))) return rc;
 
   const size_t ts = problem->dtype == CNO_F64 ? 8 : 4;
   const size_t d = (size_t)problem->d;
@@ -1178,7 +967,6 @@ int cno_minimize_host(int solver, const cno_problem_t* problem, int64_t batch, c
   local.total_ms = ms;
   local.kernel_ms = ms;
   if (info) *info = local;
-  g_last_info = local;
   return CNO_OK;
 }
 
@@ -1205,37 +993,25 @@ int cno_lbfgsb_minimize(const cno_problem_t* problem, const cno_bounds_t* bounds
   if (batch == 0) return have_device() ? CNO_OK : CNO_ERR_NO_DEVICE;
   if (!x0) return CNO_ERR_INVALID_ARGUMENT;
   if (bounds && bounds->stride != 0 && bounds->stride < problem->d) return CNO_ERR_INVALID_ARGUMENT;
-  if (!workspace || workspace_bytes < kWorkspaceBytes || ((uintptr_t)workspace & 7)) return CNO_ERR_WORKSPACE;
-  if (((uintptr_t)x0 & 15) || ((uintptr_t)out->x & 15) || ((uintptr_t)out->gradient & 15)) return CNO_ERR_INVALID_ARGUMENT;
-  cno_stop_t dflt;
-  if (!stop) { cno_lbfgsb_default_stop(&dflt); stop = &dflt; }
-  if (stop->past > CNO_MAX_PAST || stop->past < 0) return CNO_ERR_INVALID_ARGUMENT;
+  if (!queue_workspace_ok(workspace, workspace_bytes)) return CNO_ERR_WORKSPACE;
+  if (!io_aligned(x0, out)) return CNO_ERR_INVALID_ARGUMENT;
+  cno_stop_t local;
+  int rc = resolve_stop(stop, &local, cno_lbfgsb_default_stop);
+  if (rc) return rc;
   if (!have_device()) return CNO_ERR_NO_DEVICE;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  EventOwner e0, e1;
-  if (info) {
-    CNO_CUDA(e0.create());
-    CNO_CUDA(e1.create());
-    CNO_CUDA(cudaEventRecord(e0.e, s));
-  }
+  cno::LaunchTimer timer(s, info);
+  if ((rc = timer.start(g_last_cuda))) return rc;
   const LbfgsbArgs a{problem, bounds, (long long)batch, x0, stop, out, workspace, s, info};
-  const int rc = e->fn(a);
-  if (rc) return rc;
-  if (info) {
-    CNO_CUDA(cudaEventRecord(e1.e, s));
-    CNO_CUDA(cudaEventSynchronize(e1.e));
-    CNO_CUDA(cudaEventElapsedTime(&info->kernel_ms, e0.e, e1.e));
-    info->total_ms = info->kernel_ms;
-  }
-  return CNO_OK;
+  if ((rc = e->fn(a))) return rc;
+  return timer.stop(g_last_cuda);
 }
 
 int cno_evaluate(const cno_problem_t* problem, int64_t batch, const void* x, void* value, void* gradient,
                  void* stream) {
   if (!problem || batch < 0) return CNO_ERR_INVALID_ARGUMENT;
   if (problem->dtype != CNO_F64 && problem->dtype != CNO_F32) return CNO_ERR_INVALID_ARGUMENT;
-  const int dflt = (problem->dtype == CNO_F64) ? CNO_POLICY_DMMA_TREE : CNO_POLICY_WARP_TREE;
-  if (problem->policy != dflt) return CNO_ERR_UNSUPPORTED;
+  if (problem->policy != default_policy(problem->dtype)) return CNO_ERR_UNSUPPORTED;
   for (const EvalEntry& e : kEvalTable)
     if (e.family == problem->family && e.dtype == problem->dtype && e.d == problem->d) {
       if (!have_device()) return CNO_ERR_NO_DEVICE;
@@ -1248,8 +1024,7 @@ int cno_condition_hessian(const cno_problem_t* problem, int64_t batch, const voi
                           void* workspace, size_t workspace_bytes, void* stream) {
   if (!problem || batch < 0) return CNO_ERR_INVALID_ARGUMENT;
   if (problem->dtype != CNO_F64 && problem->dtype != CNO_F32) return CNO_ERR_INVALID_ARGUMENT;
-  const int dflt = (problem->dtype == CNO_F64) ? CNO_POLICY_DMMA_TREE : CNO_POLICY_WARP_TREE;
-  if (problem->policy != dflt) return CNO_ERR_UNSUPPORTED;  // (the fused-LU policy has no condition-number kernel)
+  if (problem->policy != default_policy(problem->dtype)) return CNO_ERR_UNSUPPORTED;  // (the fused-LU policy has no condition-number kernel)
   for (const CondEntry& e : kCondTable)
     if (e.family == problem->family && e.dtype == problem->dtype && e.d == problem->d) {
       if (batch == 0) return CNO_OK;
@@ -1287,7 +1062,7 @@ int cno_fill_uniform(int dtype, void* dst, int64_t first, int64_t count, uint64_
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int block = 256;
   int sms = 0;
-  const int rc = device_sm_count(&sms);
+  const int rc = cno::device_sm_count(&sms, g_last_cuda);
   if (rc) return rc;
   long long blocks = (count + block - 1) / block;
   if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;  // grid-stride loop: 16 blocks per SM
@@ -1466,31 +1241,19 @@ int cno_al_minimize(const cno_problem_t* objective, const cno_constraints_t* con
                    (size_t)constraints->n_ineq, ts);
   if (!workspace || workspace_bytes < L.total || ((uintptr_t)workspace & 255)) return CNO_ERR_WORKSPACE;
   cno_stop_t idflt;
-  if (!inner_stop) { cno_default_stop(&idflt); inner_stop = &idflt; }
-  if (inner_stop->past > CNO_MAX_PAST || inner_stop->past < 0) return CNO_ERR_INVALID_ARGUMENT;
+  if ((rc = resolve_stop(inner_stop, &idflt, cno_default_stop))) return rc;
   cno_al_stop_t odflt;
   if (!outer_stop) { cno_al_default_stop(&odflt); outer_stop = &odflt; }
   cno_al_config_t cdflt;
   if (!config) { cno_al_default_config(&cdflt); config = &cdflt; }
   if (!have_device()) return CNO_ERR_NO_DEVICE;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  EventOwner e0, e1;
-  if (info) {
-    CNO_CUDA(e0.create());
-    CNO_CUDA(e1.create());
-    CNO_CUDA(cudaEventRecord(e0.e, s));
-  }
+  cno::LaunchTimer timer(s, info);
+  if ((rc = timer.start(g_last_cuda))) return rc;
   const AlArgs a{objective, constraints, (long long)batch, x0, eq0, ineq0, penalty0, inner_stop,
                  outer_stop, config, out, static_cast<unsigned char*>(workspace), s, info};
-  rc = al_find(objective)->fn(a);
-  if (rc) return rc;
-  if (info) {
-    CNO_CUDA(cudaEventRecord(e1.e, s));
-    CNO_CUDA(cudaEventSynchronize(e1.e));
-    CNO_CUDA(cudaEventElapsedTime(&info->total_ms, e0.e, e1.e));
-    info->kernel_ms = info->total_ms;
-  }
-  return CNO_OK;
+  if ((rc = al_find(objective)->fn(a))) return rc;
+  return timer.stop(g_last_cuda);
 }
 
 }  // extern "C"

@@ -35,6 +35,8 @@ struct BfgsSmem {
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
   // register-limited: H row = D scalars per thread (64 regs at D=32 fp64)
   static constexpr int kWarps = (D * (int)sizeof(T) > 128) ? 10 : 12;
+  static constexpr int kThreads = kWarps * 32;
+  static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
 // out_i = sum_j Hrow[j] * v_j with v broadcast from shared memory (v_s[j]).
@@ -192,6 +194,8 @@ struct BfgsBigSmem {
   static constexpr int kFit = (int)((size_t)(227 * 1024) / kWarpBytes);
   static_assert(kFit >= 1, "BFGS: the inverse Hessian does not fit one SM's shared memory");
   static constexpr int kWarps = kFit > 8 ? 8 : kFit;
+  static constexpr int kThreads = kWarps * 32;
+  static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
 template <class Fn, class LS = LsMoreThuente>
@@ -366,6 +370,19 @@ bfgs_smem_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x
     __syncwarp();
   }
 }
+
+// The kernel of Bfgs<Fn> with line search LS and its plan: the inverse Hessian in registers for D <= 32, in shared
+// memory above.
+template <class Fn, class LS, bool kBig = (Fn::Dim > 32)>
+struct BfgsPlan {
+  using SM = BfgsSmem<typename Fn::Scalar, Fn::Dim>;
+  static auto kernel() { return bfgs_minimize_kernel<Fn, LS>; }
+};
+template <class Fn, class LS>
+struct BfgsPlan<Fn, LS, true> {
+  using SM = BfgsBigSmem<typename Fn::Scalar, Fn::Dim>;
+  static auto kernel() { return bfgs_smem_minimize_kernel<Fn, LS>; }
+};
 
 }  // namespace cno
 

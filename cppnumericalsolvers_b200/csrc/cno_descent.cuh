@@ -34,6 +34,8 @@ struct DescentSmem {
   static constexpr int kWarpElems = CNO_MAX_PAST;
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
   static constexpr int kWarps = 16;
+  static constexpr int kThreads = kWarps * 32;
+  static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
 // kConjugate = false: GradientDescent (MoreThuente); true: ConjugatedGradientDescent (Armijo<F,1>)

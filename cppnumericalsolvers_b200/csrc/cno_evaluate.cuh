@@ -5,6 +5,7 @@
 #define CNO_EVALUATE_CUH_
 
 #include "cno_device.cuh"
+#include "cno_launch.cuh"
 #include "../../include/cno.h"
 
 namespace cno {
@@ -39,9 +40,9 @@ inline int launch_evaluate(const Fn& fn, int64_t batch, const void* x, void* val
   if (batch < 0 || (!value && !gradient)) return CNO_ERR_INVALID_ARGUMENT;
   if (batch == 0) return CNO_OK;
   if (!x || ((uintptr_t)x & 15) || ((uintptr_t)gradient & 15)) return CNO_ERR_INVALID_ARGUMENT;
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return CNO_ERR_NO_DEVICE;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  cudaError_t last_error = cudaSuccess;
+  int sms = 0;
+  if (device_sm_count(&sms, last_error)) return CNO_ERR_NO_DEVICE;
   long long ctas = (batch + kEvalWarps - 1) / kEvalWarps;
   const long long cap = (long long)sms * 8;
   const int grid = (int)(ctas < cap ? ctas : cap);

@@ -61,6 +61,7 @@ struct LbfgsSmem {
   // warp kHelperBase + t.
   static constexpr int kHelperBase = kWarps;
   static constexpr int kThreads = 32 * (kHelpers > 0 ? 2 * kWarps : kWarps);
+  static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
 // y-history accessor: the warp's shared-memory slice (chunk-interleaved).  A load is issued before the reduction it

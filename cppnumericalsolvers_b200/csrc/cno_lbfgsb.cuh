@@ -57,6 +57,8 @@ struct LbfgsbSmem {
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
   static constexpr int kFit = (int)((size_t)(227 * 1024) / kWarpBytes);
   static constexpr int kWarps = kFit > 12 ? 12 : (kFit < 1 ? 1 : kFit);
+  static constexpr int kThreads = kWarps * 32;
+  static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
 // warp minimum of POSITIVE values by (value, index): returns the index of the smallest value, ties to the smaller

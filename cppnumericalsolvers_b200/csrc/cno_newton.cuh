@@ -384,6 +384,8 @@ struct NewtonSmem {
   static constexpr int kWarpsFit = (int)(kMaxSmem / kWarpBytes);
   static constexpr int kCap = 8;
   static constexpr int kWarps = kWarpsFit > kCap ? kCap : (kWarpsFit < 1 ? 1 : kWarpsFit);
+  static constexpr int kThreads = kWarps * 32;
+  static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
 // One elimination step's trailing update over the SHARED-MEMORY columns [j0, j1).
@@ -888,6 +890,8 @@ struct ConditionSmem {
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
   static constexpr int kWarpsFit = (int)(NS::kMaxSmem / kWarpBytes);
   static constexpr int kWarps = kWarpsFit > NS::kCap ? NS::kCap : (kWarpsFit < 1 ? 1 : kWarpsFit);
+  static constexpr int kThreads = kWarps * 32;
+  static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
 // binary tree over a column's D = 64 squared entries (lane l holds rows 2l, 2l+1), the result in every lane

@@ -469,6 +469,7 @@ struct NewtonDmmaSmem {
   static constexpr int kWarpElems = FragStore::kElems + kVecElems;
   static_assert(kWarpElems % 2 == 0, "warp slices stay 16-byte aligned");
   static constexpr int kWarps = 6;
+  static constexpr int kThreads = kWarps * 32;
   static constexpr size_t kBytes = (size_t)kWarps * kWarpElems * sizeof(double);
   static_assert(kBytes <= 227 * 1024, "shared memory per CTA");
 };

@@ -39,11 +39,12 @@
 #include "cno_bfgs.cuh"
 #include "cno_descent.cuh"
 #include "cno_evaluate.cuh"
+#include "cno_launch.cuh"
 #include "cno_lbfgs.cuh"
 #include "cno_newton.cuh"
 
 namespace cno {
-template <class Fn, class Smem, class Kernel, class... Extra>
+template <class Fn, class Plan, class Kernel, class... Extra>
 inline int launch_user(Kernel kernel, const Fn& fn, int64_t batch, const void* x0,
                        const cno_stop_t* stop, const cno_batch_out_t* out, void* workspace,
                        size_t workspace_bytes, void* stream, cno_launch_info_t* info, Extra... extra) {
@@ -58,40 +59,17 @@ inline int launch_user(Kernel kernel, const Fn& fn, int64_t batch, const void* x
   if (!stop) { cno_default_stop(&dflt); stop = &dflt; }
   // the kernels' past-f ring is CNO_MAX_PAST warp-private scalars (same check as cno_minimize)
   if (stop->past > CNO_MAX_PAST || stop->past < 0) return CNO_ERR_INVALID_ARGUMENT;
-  int dev = 0, sms = 0;
+  int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return CNO_ERR_NO_DEVICE;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const size_t smem = Smem::kWarpBytes * Smem::kWarps;
-  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-    return CNO_ERR_CUDA;
-  long long ctas = (batch + Smem::kWarps - 1) / Smem::kWarps;
-  const int grid = (int)(ctas < sms ? ctas : sms);
+  cudaError_t last_error = cudaSuccess;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaMemsetAsync(workspace, 0, 8, s);
-  struct Event {  // released on every return path
-    cudaEvent_t e = nullptr;
-    ~Event() { if (e) cudaEventDestroy(e); }
-  } e0, e1;
-  if (info) {
-    if (cudaEventCreate(&e0.e) != cudaSuccess || cudaEventCreate(&e1.e) != cudaSuccess) return CNO_ERR_CUDA;
-    cudaEventRecord(e0.e, s);
-  }
-  kernel<<<grid, Smem::kWarps * 32, smem, s>>>(fn, static_cast<const T*>(x0), (long long)batch,
-                                               make_stop<T>(*stop), make_out<T>(*out),
-                                               static_cast<unsigned long long*>(workspace), extra...);
-  if (cudaGetLastError() != cudaSuccess) return CNO_ERR_CUDA;
-  if (info) {
-    cudaEventRecord(e1.e, s);
-    if (cudaEventSynchronize(e1.e) != cudaSuccess) return CNO_ERR_CUDA;
-    cudaEventElapsedTime(&info->kernel_ms, e0.e, e1.e);
-    info->total_ms = info->kernel_ms;
-    info->kernel_launches = 1;
-    info->grid = grid;
-    info->block = Smem::kWarps * 32;
-    info->warps_per_cta = Smem::kWarps;
-    info->dynamic_smem = (int64_t)smem;
-  }
-  return CNO_OK;
+  unsigned long long* queue = static_cast<unsigned long long*>(workspace);
+  LaunchTimer timer(s, info);
+  int rc = timer.start(last_error);
+  if (!rc)
+    rc = launch_persistent<Plan>(kernel, (long long)batch, queue, s, info, last_error, fn, static_cast<const T*>(x0),
+                                 (long long)batch, make_stop<T>(*stop), make_out<T>(*out), queue, extra...);
+  return rc ? rc : timer.stop(last_error);
 }
 // ---- which optional members a functor has ----
 template <class F, class = void>
@@ -127,13 +105,8 @@ inline int user_lbfgs(const F& fn, int mode, int lbfgs_m, int64_t batch, const v
 template <class F, class LS>
 inline int user_bfgs(const F& fn, int64_t batch, const void* x0, const cno_stop_t* stop, const cno_batch_out_t* out,
                      void* workspace, size_t workspace_bytes, void* stream, cno_launch_info_t* info) {
-  if constexpr (F::Dim <= 32) {  // the register-resident inverse Hessian (cno_bfgs.cuh)
-    return launch_user<F, BfgsSmem<typename F::Scalar, F::Dim>>(bfgs_minimize_kernel<F, LS>, fn, batch, x0, stop, out,
-                                                                 workspace, workspace_bytes, stream, info);
-  } else {  // the inverse Hessian in shared memory
-    return launch_user<F, BfgsBigSmem<typename F::Scalar, F::Dim>>(bfgs_smem_minimize_kernel<F, LS>, fn, batch, x0, stop,
-                                                                    out, workspace, workspace_bytes, stream, info);
-  }
+  using P = BfgsPlan<F, LS>;
+  return launch_user<F, typename P::SM>(P::kernel(), fn, batch, x0, stop, out, workspace, workspace_bytes, stream, info);
 }
 
 template <class F>
@@ -157,24 +130,18 @@ inline int user_condition(const F& fn, int64_t batch, const void* x, void* condi
   if constexpr (F::Mode == 2 && HasHessCol<F>::value) {
     using A = SecondOrderAdapter<F>;
     using T = typename F::Scalar;
-    using CS = ConditionSmem<T, F::Dim>;
     if (batch < 0) return CNO_ERR_INVALID_ARGUMENT;
     if (batch == 0) return CNO_OK;
     if (!x || !condition || !workspace || workspace_bytes < sizeof(unsigned long long) || ((uintptr_t)workspace & 7))
       return CNO_ERR_INVALID_ARGUMENT;
-    int dev = 0, sms = 0;
+    int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return CNO_ERR_NO_DEVICE;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    auto kernel = condition_hessian_kernel<A>;
-    const size_t smem = CS::kWarpBytes * CS::kWarps;
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return CNO_ERR_CUDA;
-    long long ctas = (batch + CS::kWarps - 1) / CS::kWarps;
-    const int grid = (int)(ctas < sms ? (ctas < 1 ? 1 : ctas) : sms);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    cudaError_t last_error = cudaSuccess;
     unsigned long long* queue = static_cast<unsigned long long*>(workspace);
-    if (cudaMemsetAsync(queue, 0, sizeof(unsigned long long), s) != cudaSuccess) return CNO_ERR_CUDA;
-    kernel<<<grid, CS::kWarps * 32, smem, s>>>(A{fn}, static_cast<const T*>(x), (long long)batch, static_cast<T*>(condition), queue);
-    return cudaGetLastError() == cudaSuccess ? CNO_OK : CNO_ERR_CUDA;
+    return launch_persistent<ConditionSmem<T, F::Dim>>(condition_hessian_kernel<A>, (long long)batch, queue,
+                                                       static_cast<cudaStream_t>(stream), nullptr, last_error, A{fn},
+                                                       static_cast<const T*>(x), (long long)batch,
+                                                       static_cast<T*>(condition), queue);
   } else {
     return CNO_ERR_UNSUPPORTED;  // defined for second-order differentiable functions
   }
