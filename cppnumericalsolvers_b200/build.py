@@ -48,28 +48,34 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
 def build_cpp_tests(verbose: bool = False) -> list:
     """Compiles the C++ host-API programs under tests/cpp (g++ and nvcc translation
-    units) into tests/cpp/build/ (git-ignored)."""
+    units) into tests/cpp/build/ (git-ignored).  A program newer than its source and every header it can include
+    is left alone, so the tests that call this can run from a tree they may only read once it has been built."""
     root = os.path.dirname(HERE)
     src = os.path.join(root, "tests", "cpp")
     out = os.path.join(src, "build")
+    inc_dir = os.path.join(root, "include")
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + \
+           [os.path.join(inc_dir, f) for f in os.listdir(inc_dir) if f.endswith(".h")] + \
+           [os.path.join(inc_dir, "cppoptlib_b200", f) for f in os.listdir(os.path.join(inc_dir, "cppoptlib_b200"))]
+
+    def current(source, target):
+        return os.path.exists(target) and all(os.path.getmtime(d) <= os.path.getmtime(target) for d in deps + [source])
+
     os.makedirs(out, exist_ok=True)
     cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-    inc = ["-I" + os.path.join(root, "include"), "-I" + CSRC, f"-I{cuda}/include"]
+    inc = ["-I" + inc_dir, "-I" + CSRC, f"-I{cuda}/include"]
     link = [f"-L{HERE}", "-lcno", f"-L{cuda}/lib64", "-lcudart", f"-Wl,-rpath,{HERE}", f"-Wl,-rpath,{cuda}/lib64"]
     exes = []
-    cmd = ["g++", "-std=c++17", "-O2", "-Wall", os.path.join(src, "verify_host.cc"), *inc,
-           "-o", os.path.join(out, "verify_host"), *link]
-    subprocess.run(cmd, check=True)
-    exes.append(os.path.join(out, "verify_host"))
-    # the constrained C++ mirror (run by tests/test_al_gpu.py)
-    cmd = ["g++", "-std=c++17", "-O2", "-Wall", os.path.join(src, "al_host.cc"), *inc,
-           "-o", os.path.join(out, "al_host"), *link]
-    subprocess.run(cmd, check=True)
-    # the multi-GPU path below Python: MinimizeSharded + cno_allgather_done (NCCL resolved with dlopen)
-    cmd = ["g++", "-std=c++17", "-O2", "-Wall", "-pthread", os.path.join(src, "sharded_nccl.cc"), *inc,
-           "-o", os.path.join(out, "sharded_nccl"), *link, "-ldl"]
-    subprocess.run(cmd, check=True)
-    exes.append(os.path.join(out, "sharded_nccl"))
+    # verify_host; the constrained C++ mirror (run by tests/test_al_gpu.py); the multi-GPU path below Python:
+    # MinimizeSharded + cno_allgather_done (NCCL resolved with dlopen)
+    for name, extra, extra_link, listed in (("verify_host", [], [], True), ("al_host", [], [], False),
+                                            ("sharded_nccl", ["-pthread"], ["-ldl"], True)):
+        source, target = os.path.join(src, name + ".cc"), os.path.join(out, name)
+        if not current(source, target):
+            cmd = ["g++", "-std=c++17", "-O2", "-Wall", *extra, source, *inc, "-o", target, *link, *extra_link]
+            subprocess.run(cmd, check=True)
+        if listed:
+            exes.append(target)
     nvcc = os.environ.get("NVCC", f"{cuda}/bin/nvcc")
     xlink = ["-Xlinker", f"-rpath={HERE}"]
     dev_flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -78,11 +84,9 @@ def build_cpp_tests(verbose: bool = False) -> list:
             # user functors + composites as a shared library for the Python parity tests (tests/usertest_binding.py)
             (os.path.join(src, "user_functions.cu"), os.path.join(out, "libcno_usertest.so"),
              ["-shared", "-Xcompiler", "-fPIC"])]
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + \
-           [os.path.join(root, "include", "cppoptlib_b200", f) for f in os.listdir(os.path.join(root, "include", "cppoptlib_b200"))]
     procs = []
     for source, target, extra in jobs:
-        if os.path.exists(target) and all(os.path.getmtime(d) <= os.path.getmtime(target) for d in deps + [source]):
+        if current(source, target):
             continue
         procs.append(subprocess.Popen([nvcc, *dev_flags, *extra, source, *inc, "-o", target, f"-L{HERE}", "-lcno", *xlink]))
     for p in procs:

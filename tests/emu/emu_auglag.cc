@@ -14,6 +14,9 @@
 #include "cno_newton_dmma.cuh"
 #include "cno_lbfgsb.cuh"
 #include "cno_logistic.cuh"
+#include "cno_evaluate.cuh"
+
+#define CNO_EMU_COMMA ,
 
 namespace {
 
@@ -322,6 +325,48 @@ extern "C" int emu_logistic_evaluate(const cno_problem_t* p, long long batch, co
   return 0;
 }
 
+// cno_evaluate under emulation: evaluate_kernel (csrc/cno_evaluate.cuh) as one CTA of kEvalWarps warps, run one
+// after the other, on the functors of kEvalTable (csrc/cno_api.cu).  value or gradient may be null, as at the C ABI.
+template <class Fn>
+int run_evaluate(const Fn& fn, long long B, const void* x, void* value, void* gradient) {
+  using T = typename Fn::Scalar;
+  for (int w = 0; w < cno::kEvalWarps; ++w)
+    emu::run_warp([&](int lane) {
+      gridDim.x = 1;
+      blockIdx.x = 0;
+      threadIdx.x = (unsigned)(32 * w + lane);
+      cno::evaluate_kernel<Fn>(fn, (const T*)x, B, (T*)value, (T*)gradient);
+    });
+  return 0;
+}
+
+extern "C" int emu_evaluate(const cno_problem_t* p, long long batch, const void* x, void* value, void* gradient) {
+#define EVAL_CASE(FAM, DT, TY, DIM, FN)                               \
+  if (p->family == FAM && p->dtype == DT && p->d == DIM) return run_evaluate(cno::FN, batch, x, value, gradient);
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F64, double, 2, RosenbrockFn<double CNO_EMU_COMMA 2>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F64, double, 3, RosenbrockFn<double CNO_EMU_COMMA 3>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F64, double, 8, RosenbrockFn<double CNO_EMU_COMMA 8>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F64, double, 32, RosenbrockFn<double CNO_EMU_COMMA 32>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F64, double, 37, RosenbrockFn<double CNO_EMU_COMMA 37>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F64, double, 64, RosenbrockFn<double CNO_EMU_COMMA 64>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F64, double, 128, RosenbrockFn<double CNO_EMU_COMMA 128>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F32, float, 2, RosenbrockFn<float CNO_EMU_COMMA 2>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F32, float, 32, RosenbrockFn<float CNO_EMU_COMMA 32>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F32, float, 37, RosenbrockFn<float CNO_EMU_COMMA 37>{})
+  EVAL_CASE(CNO_FN_ROSENBROCK, CNO_F32, float, 128, RosenbrockFn<float CNO_EMU_COMMA 128>{})
+  EVAL_CASE(CNO_FN_DIAG_QUADRATIC, CNO_F64, double, 2, DiagQuadraticFn<double>{})
+  EVAL_CASE(CNO_FN_HALF_SQUARED_NORM, CNO_F64, double, 2, HalfSquaredNormFn<double CNO_EMU_COMMA 2>{})
+  EVAL_CASE(CNO_FN_HALF_SQUARED_NORM, CNO_F64, double, 8, HalfSquaredNormFn<double CNO_EMU_COMMA 8>{})
+  EVAL_CASE(CNO_FN_HALF_SQUARED_NORM, CNO_F64, double, 50, HalfSquaredNormFn<double CNO_EMU_COMMA 50>{})
+  const double* data = (const double*)p->data;
+  const long long stride = (long long)p->data_stride;
+  EVAL_CASE(CNO_FN_DENSE_QUADRATIC, CNO_F64, double, 2, DenseQuadraticGlobalFn<double CNO_EMU_COMMA 2>{data CNO_EMU_COMMA stride})
+  EVAL_CASE(CNO_FN_DENSE_QUADRATIC, CNO_F64, double, 8, DenseQuadraticGlobalFn<double CNO_EMU_COMMA 8>{data CNO_EMU_COMMA stride})
+  EVAL_CASE(CNO_FN_DENSE_QUADRATIC, CNO_F64, double, 64, DenseQuadraticGlobalFn<double CNO_EMU_COMMA 64>{data CNO_EMU_COMMA stride})
+#undef EVAL_CASE
+  return CNO_ERR_UNSUPPORTED;
+}
+
 // ---- cno::al_outer_loop (csrc/cno_auglag_host.h: the host side of cno_al_minimize) with an emulation backend ----
 template <class Obj>
 struct AlEmuBackend {
@@ -462,7 +507,6 @@ extern "C" int emu_al(int op, const cno_problem_t* objective, const cno_constrai
 }
 
 
-#define CNO_EMU_COMMA ,
 // Lbfgsb<F, 5> (csrc/cno_lbfgsb.cuh) under emulation.  lower / upper: host arrays [d] (stride 0) or [B, d].
 template <class Fn, int M = 5>
 int run_lbfgsb(long long B, const void* x0, const void* lower, const void* upper, long long stride, const cno_stop_t* stop,

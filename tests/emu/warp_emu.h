@@ -162,7 +162,7 @@ inline void run_team(const std::function<void(int, int)>& f) {
 }
 }  // namespace emu
 
-inline thread_local emu::Dim3 threadIdx, blockIdx;
+inline thread_local emu::Dim3 threadIdx, blockIdx, gridDim;
 
 template <class T> inline T __shfl_sync(unsigned, T v, int src) { return emu::exchange(v, src); }
 template <class T> inline T __shfl_xor_sync(unsigned, T v, int m) { return emu::exchange(v, emu::tl_lane ^ m); }

@@ -16,6 +16,7 @@ import glob
 import os
 import subprocess
 
+import edge_sums as es
 import numpy as np
 import pytest
 
@@ -614,6 +615,43 @@ def test_emulated_al_reference_kkt_known_answers_on_the_device_path(emu):
     assert abs(x[0] - 0.5) <= 1e-3 and abs(x[1] - 1.5) <= 1e-3 and 2.0 - (x[0] + x[1]) >= -1e-5
     assert r["inequality_multipliers"][0, 0] >= -1e-2
     _assert_same(r, ob.al_minimize(*args, data=data, **kw))
+
+
+def emulated_evaluate(emu, family, x, data=None, value=True, gradient=True):
+    """cno_evaluate's kernel (csrc/cno_evaluate.cuh: evaluate_kernel) under emulation; unrequested outputs are None."""
+    x = np.ascontiguousarray(x)
+    B = x.shape[0]
+    prob = _problem(family, x, data=data)
+    f = np.zeros(B, x.dtype) if value else None
+    g = np.zeros_like(x) if gradient else None
+    emu.emu_evaluate.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]
+    assert emu.emu_evaluate(C.byref(prob), B, x.ctypes.data, _ptr(f), _ptr(g)) == 0
+    return f, g
+
+
+@pytest.mark.parametrize("case", es.probe_cases(), ids=lambda c: c[0])
+def test_emulated_evaluate_edge_vectors_equal_model_and_oracle(emu, case):
+    """The summation edges of tests/test_evaluate_gpu.py (subnormal partials and results, overflow in each stage of the
+    tensor-core tree, absorption, +-Inf, a NaN in every lane, -0.0; fp32 Rosenbrock with a subnormal gradient, an
+    overflowing value, NaN starts) on the device source under emulation: emulated kernel == numpy model of the
+    specification == oracle, bit for bit (NaN: NaN-ness only).  A later difference on the GPU is then the hardware's."""
+    name, family, x, data, names, (fm, gm) = case
+    fo, go = ob.evaluate(family, x, data=data)
+    f, g = emulated_evaluate(emu, family, x, data)
+    for i, vec in enumerate(names):
+        assert es.same_bits(f[i], fm[i]) and es.same_bits(fo[i], fm[i]), (vec, f[i], fm[i], fo[i])
+        assert es.same_bits(g[i], gm[i]) and es.same_bits(go[i], gm[i]), vec
+    ok = es.chain_finite(family, x, data)
+    assert ok.any()
+    es.check_exact(family, x[ok], None if data is None else data[ok], f[ok], g[ok], x.dtype.type)
+    if name.startswith("rosenbrock"):
+        k = names.index("subnormal_gradient")
+        assert g[k, -1] == es.SUBNORMAL_G != 0 and abs(g[k, -1]) < np.finfo(np.float32).tiny
+        k = names.index("huge")
+        assert f[k] == np.inf and np.isfinite(g[k]).all()
+    f1, _ = emulated_evaluate(emu, family, x, data, gradient=False)
+    _, g1 = emulated_evaluate(emu, family, x, data, value=False)
+    assert es.same_bits(f1, f) and es.same_bits(g1, g)
 
 
 @pytest.mark.parametrize("d,B,hz", [(37, 4, 0), (128, 2, 0), (37, 3, 1)])
