@@ -18,7 +18,6 @@
 #include "cno_al_oracle.h"
 #include "cno_oracle.h"
 
-#define CNO_ORACLE_MAX_M 32
 static inline int problem_lbfgs_m(const cno_problem_t* p) {
   return (p->lbfgs_m > 0 && p->lbfgs_m <= CNO_ORACLE_MAX_M) ? p->lbfgs_m : CNO_LBFGS_M;
 }
@@ -112,9 +111,9 @@ int cno_oracle_minimize(int solver, const cno_problem_t* problem, int64_t batch,
   return cno_oracle_minimize_ls(solver, problem, batch, x0, stop, out, threads, CNO_LS_MORE_THUENTE);
 }
 
-int cno_oracle_minimize_ls(int solver, const cno_problem_t* problem, int64_t batch,
-                           const void* x0, const cno_stop_t* stop,
-                           const cno_batch_out_t* out, int threads, int linesearch) {
+static int minimize_batch(int solver, const cno_problem_t* problem, int64_t batch, const void* x0,
+                          const cno_stop_t* stop, const cno_batch_out_t* out, int threads, int linesearch,
+                          cno_lbfgs_paths_t* paths) {
   int rc = check_problem(solver, problem);
   if (linesearch != CNO_LS_MORE_THUENTE && linesearch != CNO_LS_HAGER_ZHANG) return CNO_ERR_INVALID_ARGUMENT;
   if (linesearch == CNO_LS_HAGER_ZHANG && solver != CNO_LBFGS && solver != CNO_BFGS &&
@@ -146,7 +145,7 @@ int cno_oracle_minimize_ls(int solver, const cno_problem_t* problem, int64_t bat
           out->status ? out->status + b : NULL, out->nfev ? out->nfev + b : NULL,
           out->x_delta ? (double*)out->x_delta + b : NULL,
           out->f_delta ? (double*)out->f_delta + b : NULL,
-          out->gradient_norm ? (double*)out->gradient_norm + b : NULL);
+          out->gradient_norm ? (double*)out->gradient_norm + b : NULL, paths ? paths + b : NULL);
     } else {
       minimize_one_f32(
           solver, problem, NULL, linesearch, b, (const float*)x0 + b * d, stop,
@@ -157,10 +156,24 @@ int cno_oracle_minimize_ls(int solver, const cno_problem_t* problem, int64_t bat
           out->status ? out->status + b : NULL, out->nfev ? out->nfev + b : NULL,
           out->x_delta ? (float*)out->x_delta + b : NULL,
           out->f_delta ? (float*)out->f_delta + b : NULL,
-          out->gradient_norm ? (float*)out->gradient_norm + b : NULL);
+          out->gradient_norm ? (float*)out->gradient_norm + b : NULL, paths ? paths + b : NULL);
     }
   }
   return CNO_OK;
+}
+
+int cno_oracle_minimize_ls(int solver, const cno_problem_t* problem, int64_t batch,
+                           const void* x0, const cno_stop_t* stop,
+                           const cno_batch_out_t* out, int threads, int linesearch) {
+  return minimize_batch(solver, problem, batch, x0, stop, out, threads, linesearch, NULL);
+}
+
+int cno_oracle_lbfgs_paths(const cno_problem_t* problem, int64_t batch, const void* x0,
+                           const cno_stop_t* stop, const cno_batch_out_t* out,
+                           cno_lbfgs_paths_t* paths, int threads) {
+  if (!paths) return CNO_ERR_INVALID_ARGUMENT;
+  if (batch > 0) memset(paths, 0, sizeof(*paths) * (size_t)batch);
+  return minimize_batch(CNO_LBFGS, problem, batch, x0, stop, out, threads, CNO_LS_MORE_THUENTE, paths);
 }
 
 int cno_oracle_evaluate(const cno_problem_t* problem, int64_t batch,
@@ -383,13 +396,13 @@ int cno_al_oracle_inner_minimize(const cno_problem_t* objective, const cno_const
                               ineq ? (const double*)ineq + b * ni : NULL, ((const double*)penalty)[b]};
       minimize_one_f64(CNO_LBFGS, objective, &al, 0, b, (const double*)x0 + b * d, inner_stop,
                        (double*)x_out + b * d, NULL, NULL, NULL, NULL, nfev_out ? nfev_out + b : NULL, NULL,
-                       NULL, NULL);
+                       NULL, NULL, NULL);
     } else {
       const alctx_t_f32 al = {constraints, eq ? (const float*)eq + b * ne : NULL,
                               ineq ? (const float*)ineq + b * ni : NULL, ((const float*)penalty)[b]};
       minimize_one_f32(CNO_LBFGS, objective, &al, 0, b, (const float*)x0 + b * d, inner_stop,
                        (float*)x_out + b * d, NULL, NULL, NULL, NULL, nfev_out ? nfev_out + b : NULL, NULL,
-                       NULL, NULL);
+                       NULL, NULL, NULL);
     }
   }
   return CNO_OK;

@@ -40,6 +40,28 @@ int cno_oracle_minimize_ls(int solver, const cno_problem_t* problem, int64_t bat
                            const void* x0, const cno_stop_t* stop,
                            const cno_batch_out_t* out, int threads, int linesearch);
 
+/* Most pairs Lbfgs<F, m> may keep (cno_problem_t::lbfgs_m). */
+#define CNO_ORACLE_MAX_M 32
+
+/* How often one Lbfgs instance took the rare branches of OptimizationStep (lbfgs.h:89-303), so that tests can show
+ * which paths an input reaches.  k = mem_count when the step begins. */
+typedef struct cno_lbfgs_paths {
+  /* pairs skipped by the first loop (|s_i . y_i| < eps, lbfgs.h:165): [k < m, k == m][position counted from the
+   * newest pair: 0, 1, >= 2] */
+  uint64_t skipped[2][3];
+  /* pairs refused by the curvature test (lbfgs.h:267) while the history held at least one pair */
+  uint64_t rejected;
+  /* descent-test fallbacks (lbfgs.h:214-224), by k */
+  uint64_t fallback[CNO_ORACLE_MAX_M + 1];
+  /* non-finite line-search results (lbfgs.h:239-241), by k after the descent test */
+  uint64_t nonfinite[CNO_ORACLE_MAX_M + 1];
+} cno_lbfgs_paths_t;
+
+/* cno_oracle_minimize(CNO_LBFGS, ...) with MoreThuente that also fills paths[batch]. */
+int cno_oracle_lbfgs_paths(const cno_problem_t* problem, int64_t batch, const void* x0,
+                           const cno_stop_t* stop, const cno_batch_out_t* out,
+                           cno_lbfgs_paths_t* paths, int threads);
+
 /* HagerZhang<F,1>::Search on the 1-D quartic (((c4 v + c3) v + c2) v + c1) v + c0 of
  * src/test/hager_zhang_test.cc (Quadratic, Cubic, FlatQuartic) along s = +1 from x0. */
 int cno_oracle_hz_search_poly(const double coef[5], double x0, double alpha_init,

@@ -102,6 +102,15 @@ def _np_dtype(a):
 LS_MORE_THUENTE, LS_HAGER_ZHANG = 0, 1
 
 
+def _batch_out(x0: np.ndarray):
+    B, dt = x0.shape[0], x0.dtype
+    r = dict(x=np.zeros_like(x0), value=np.zeros(B, dt), gradient=np.zeros_like(x0),
+             num_iterations=np.zeros(B, np.uint32), status=np.zeros(B, np.int8),
+             nfev=np.zeros(B, np.uint32), x_delta=np.zeros(B, dt), f_delta=np.zeros(B, dt),
+             gradient_norm=np.zeros(B, dt))
+    return r, BatchOut(*[r[k].ctypes.data for k, _ in BatchOut._fields_])
+
+
 def minimize(solver: int, family: int, x0: np.ndarray, *, policy: int | None = None, stop: Stop | None = None,
              data: np.ndarray | None = None, n: int = 0, param: float = 0.0, threads: int = 0,
              impl: str = "oracle", mode: int = 0, linesearch: int = LS_MORE_THUENTE, lbfgs_m: int = 0) -> dict:
@@ -118,13 +127,7 @@ def minimize(solver: int, family: int, x0: np.ndarray, *, policy: int | None = N
     p = Problem(family, _np_dtype(x0), d, n, param,
                 data.ctypes.data if data is not None else None,
                 data.shape[1] if data is not None else 0, policy, mode, lbfgs_m)
-    r = dict(x=np.zeros_like(x0), value=np.zeros(B, dt), gradient=np.zeros_like(x0),
-             num_iterations=np.zeros(B, np.uint32), status=np.zeros(B, np.int8),
-             nfev=np.zeros(B, np.uint32), x_delta=np.zeros(B, dt), f_delta=np.zeros(B, dt),
-             gradient_norm=np.zeros(B, dt))
-    o = BatchOut(*[r[k].ctypes.data for k in (
-        "x", "value", "gradient", "num_iterations", "status", "nfev", "x_delta", "f_delta",
-        "gradient_norm")])
+    r, o = _batch_out(x0)
     fn = oracle_lib().cno_oracle_minimize_ls if impl == "oracle" else ref_lib().cno_ref_minimize_ls
     t0 = time.perf_counter()
     rc = fn(solver, C.byref(p), C.c_int64(B), C.c_void_p(x0.ctypes.data),
@@ -133,6 +136,31 @@ def minimize(solver: int, family: int, x0: np.ndarray, *, policy: int | None = N
     if rc != 0:
         raise RuntimeError(f"oracle minimize failed: {rc}")
     return r
+
+
+MAX_M = 32  # CNO_ORACLE_MAX_M
+
+
+def lbfgs_paths(family: int, x0: np.ndarray, *, stop: Stop | None = None, lbfgs_m: int = 0,
+                policy: int | None = None, threads: int = 0) -> tuple[dict, dict]:
+    """minimize(LBFGS, family, x0) with MoreThuente, plus how often each instance took the rare branches of
+    OptimizationStep (cno_lbfgs_paths_t): skipped [B, 2, 3] (k < m / k == m; position 0, 1, >= 2 from the newest
+    pair), rejected [B], fallback [B, MAX_M + 1] and nonfinite [B, MAX_M + 1] (by mem_count)."""
+    x0 = np.ascontiguousarray(x0)
+    B, d = x0.shape
+    p = Problem(family, _np_dtype(x0), d, 0, 0.0, None, 0, device_policy(x0.dtype) if policy is None else policy, 0,
+                lbfgs_m)
+    r, o = _batch_out(x0)
+    n = MAX_M + 1
+    raw = np.zeros((B, 7 + 2 * n), np.uint64)
+    rc = oracle_lib().cno_oracle_lbfgs_paths(C.byref(p), C.c_int64(B), C.c_void_p(x0.ctypes.data),
+                                             C.byref(stop) if stop is not None else None, C.byref(o),
+                                             C.c_void_p(raw.ctypes.data), threads)
+    if rc != 0:
+        raise RuntimeError(f"oracle lbfgs_paths failed: {rc}")
+    paths = dict(skipped=raw[:, :6].reshape(B, 2, 3), rejected=raw[:, 6], fallback=raw[:, 7:7 + n],
+                 nonfinite=raw[:, 7 + n:])
+    return r, paths
 
 
 def evaluate(family: int, x: np.ndarray, *, policy: int | None = None, data=None, n: int = 0,

@@ -142,7 +142,7 @@ int run(const Obj& obj, int op, const cno_constraints_t* k, long long B, const E
 }  // namespace
 
 // ---- the unconstrained solver kernels under emulation (one warp draining the queue) ----
-template <class Fn, class LS>
+template <class Fn, class LS, int M = CNO_LBFGS_M>
 int run_solver(int solver, long long B, const void* x0, const cno_stop_t* stop, const cno_batch_out_t* out,
                const Fn fn = Fn{}) {
   using T = typename Fn::Scalar;
@@ -154,7 +154,7 @@ int run_solver(int solver, long long B, const void* x0, const cno_stop_t* stop, 
     const auto sp = cno::make_stop<T>(*stop);
     const auto bo = cno::make_out<T>(*out);
     if (solver == CNO_LBFGS) {
-      cno::lbfgs_minimize_kernel<Fn, CNO_LBFGS_M, false, LS>(fn, (const T*)x0, B, sp, bo, &queue, cno::ResumeArgs{nullptr, 0, 0, 0});
+      cno::lbfgs_minimize_kernel<Fn, M, false, LS>(fn, (const T*)x0, B, sp, bo, &queue, cno::ResumeArgs{nullptr, 0, 0, 0});
     } else if (solver == CNO_BFGS) {
       if constexpr (Fn::Dim <= 32) cno::bfgs_minimize_kernel<Fn, LS>(fn, (const T*)x0, B, sp, bo, &queue);
       else cno::bfgs_smem_minimize_kernel<Fn, LS>(fn, (const T*)x0, B, sp, bo, &queue);  // H in shared memory
@@ -170,9 +170,24 @@ int run_solver(int solver, long long B, const void* x0, const cno_stop_t* stop, 
 }
 
 // solver: CNO_LBFGS / CNO_BFGS / CNO_GRADIENT_DESCENT / CNO_CONJUGATED_GRADIENT_DESCENT; hager_zhang selects
-// the LineSearch policy.  Host pointers.
+// the LineSearch policy; p->lbfgs_m selects Lbfgs<F, m> (0 = the default m).  Host pointers.
 extern "C" int emu_minimize(int solver, int hager_zhang, const cno_problem_t* p, long long batch, const void* x0,
                             const cno_stop_t* stop, const cno_batch_out_t* out) {
+  // Lbfgs<F, m> for the other compiled m (lbfgs.h:40-41): at m = 20 the plan keeps two pairs in registers, at m = 5 none
+  if (solver == CNO_LBFGS && p->lbfgs_m != 0 && p->lbfgs_m != CNO_LBFGS_M) {
+    if (hager_zhang || p->family != CNO_FN_ROSENBROCK || p->dtype != CNO_F64 || p->mode == 2 ||
+        p->policy == CNO_POLICY_EIGEN_SSE2)
+      return CNO_ERR_UNSUPPORTED;
+#define LBFGS_M_CASE(DIM, M) \
+  if (p->d == DIM && p->lbfgs_m == M) \
+    return run_solver<cno::RosenbrockFn<double, DIM>, cno::LsMoreThuente, M>(solver, batch, x0, stop, out);
+    LBFGS_M_CASE(37, 5)
+    LBFGS_M_CASE(37, 20)
+    LBFGS_M_CASE(128, 5)
+    LBFGS_M_CASE(128, 20)
+#undef LBFGS_M_CASE
+    return CNO_ERR_UNSUPPORTED;
+  }
   if (solver == CNO_LBFGS && !hager_zhang && p->family == CNO_FN_DENSE_QUADRATIC && p->dtype == CNO_F64 && p->mode != 2) {
     const double* data = (const double*)p->data;
     const long long stride = (long long)p->data_stride;
