@@ -17,6 +17,7 @@
 #include "cno_functors.cuh"
 #include "cno_kernel_params.h"
 #include "cno_lbfgs.cuh"
+#include "cno_lbfgs_group.cuh"
 #include "cno_lbfgsb.cuh"
 #include "cno_bfgs.cuh"
 #include "cno_descent.cuh"
@@ -176,6 +177,15 @@ int lbfgs_rosenbrock_m(const LaunchArgs& a) { return lbfgs<cno::RosenbrockFn<T, 
 int lbfgs_rosenbrock_d128_eigen(const LaunchArgs& a) {
   return lbfgs(cno::RosenbrockFn<double, 128, cno::PolicyEigenSSE2>{}, a);
 }
+// d = 512 / 1024 fp64 (cno_lbfgs_group.cuh): one group of d / 128 warps per instance, the history in the group's shared
+// memory; MoreThuente, First mode, the default m and policy only (no stepwise variant).  No row at d = 256: there the
+// group kernel was measured slower than the one-warp kernel (DESIGN.md 2.10).
+template <int D>
+int lbfgs_group_rosenbrock(const LaunchArgs& a) {
+  using Fn = cno::GroupRosenbrockFn<double, D>;
+  return launch_solve<cno::LbfgsGroupPlan<double, D, CNO_LBFGS_M>>(cno::lbfgs_group_minimize_kernel<Fn, CNO_LBFGS_M>,
+                                                                   Fn{}, a);
+}
 // Lbfgs on a Second-mode function: diagonal-preconditioner branch (lbfgs.h:116-139)
 template <class T, int D>
 int lbfgs_rosenbrock_second(const LaunchArgs& a) {
@@ -278,6 +288,8 @@ const Entry kTable[] = {
     {CNO_LBFGS, CNO_FN_ROSENBROCK, CNO_F64, 128, lbfgs_rosenbrock<double, 128>, -1, 0,
      lbfgs_rosenbrock_steps<double, 128>, lbfgs_state_stride<double, 128>},
     {CNO_LBFGS, CNO_FN_ROSENBROCK, CNO_F64, 128, lbfgs_rosenbrock_d128_eigen, CNO_POLICY_EIGEN_SSE2},
+    {CNO_LBFGS, CNO_FN_ROSENBROCK, CNO_F64, 512, lbfgs_group_rosenbrock<512>},
+    {CNO_LBFGS, CNO_FN_ROSENBROCK, CNO_F64, 1024, lbfgs_group_rosenbrock<1024>},
     {CNO_LBFGS, CNO_FN_ROSENBROCK, CNO_F64, 2, lbfgs_rosenbrock_second<double, 2>, -1, 2},
     {CNO_LBFGS, CNO_FN_ROSENBROCK, CNO_F64, 37, lbfgs_rosenbrock_second<double, 37>, -1, 2},
     {CNO_LBFGS, CNO_FN_ROSENBROCK, CNO_F64, 128, lbfgs_rosenbrock_second<double, 128>, -1, 2},

@@ -145,8 +145,10 @@ __device__ __forceinline__ typename LanePartial<P, T, E>::type ls_dir_dot(const 
 }
 // f(x0 +- stp*s) and g.(+-s): the trial point of every line search (more_thuente.h:198-201,
 // hager_zhang.h:152-159), f and the slope reduced together when the functor exposes its partial.
-template <bool kNeg, class Fn, class T, int E>
-__device__ __forceinline__ void ls_eval(const Fn& fn, const EvalCtx& ctx, const RedCtx<T>& rc, const T (&x0)[E],
+// RC: the reduction context -- RedCtx<T> of the one-warp kernels, or the group context of a kernel in which several
+// warps share one instance (cno_lbfgs_group.cuh); warp_sum_p / warp_sum2_p are overloaded on it.
+template <bool kNeg, class Fn, class T, int E, class RC>
+__device__ __forceinline__ void ls_eval(const Fn& fn, const EvalCtx& ctx, const RC& rc, const T (&x0)[E],
                                         const T stp, const T (&s)[E], T (&x)[E], T& f, T (&g)[E], T& dg) {
   using P = typename PolicyOf<Fn>::type;
 #pragma unroll
@@ -160,8 +162,8 @@ __device__ __forceinline__ void ls_eval(const Fn& fn, const EvalCtx& ctx, const 
   }
 }
 
-template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false>
-__device__ __forceinline__ int cvsrch(const Fn& fn, const EvalCtx& ctx, const RedCtx<T>& rc, const T (&x0)[E],
+template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false, class RC>
+__device__ __forceinline__ int cvsrch(const Fn& fn, const EvalCtx& ctx, const RC& rc, const T (&x0)[E],
                                       const T f0, const T (&g0)[E], T (&x)[E], T& f,
                                       T (&g)[E], T stp, const T (&s)[E], const T dginit) {
   int info = 0;
