@@ -26,8 +26,7 @@
 #include "cno_newton.cuh"
 #include "cno_newton_dmma.cuh"
 #include "cno_logistic.cuh"
-#include "cno_auglag.cuh"
-#include "cno_auglag_host.h"
+#include "cno_auglag_launch.cuh"
 #include "../../include/cno_al.h"
 
 namespace {
@@ -548,109 +547,29 @@ __global__ void cstep_kernel(double* io, int* flags) {
   flags[2] = ret;
 }
 
-// ---- AugmentedLagrangian (include/cno_al.h; csrc/cno_auglag.cuh) -----------------
-struct AlArgs {
-  const cno_problem_t* objective;
-  const cno_constraints_t* constraints;
-  long long batch;
-  const void* x0;
-  const void* eq0;
-  const void* ineq0;
-  const void* penalty0;
-  const cno_stop_t* inner_stop;
-  const cno_al_stop_t* outer_stop;
-  const cno_al_config_t* config;
-  const cno_al_out_t* out;
-  unsigned char* workspace;
-  cudaStream_t stream;
-  cno_launch_info_t* info;
-};
-
-using cno::AlLayout;
-
-// The CUDA backend of cno::al_outer_loop (csrc/cno_auglag_host.h).
+// ---- AugmentedLagrangian (include/cno_al.h; csrc/cno_auglag.cuh, csrc/cno_auglag_launch.cuh) ----
 template <class Obj>
-struct AlCudaBackend {
-  using T = typename Obj::Scalar;
-  const Obj& obj;
-  const AlArgs& A;
-  cno::AlArrays<T> a;
-  cno::AlView<T> view;
-  cno::AlParams<T> p;
-  unsigned char* queue;
-  cudaStream_t s;
-  int blocks, threads;
-
-  int copy_or_zero(void* dst, const void* src, size_t bytes) {
-    if (!bytes || src == dst) return CNO_OK;  // (a caller may pass its state arrays as the initial values)
-    CNO_CUDA(src ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s) : cudaMemsetAsync(dst, 0, bytes, s));
-    return CNO_OK;
-  }
-  int fill(void* dst, int byte, size_t bytes) {
-    if (bytes) CNO_CUDA(cudaMemsetAsync(dst, byte, bytes, s));
-    return CNO_OK;
-  }
-  int autoscale() {
-    cno::al_autoscale_kernel<Obj><<<blocks, threads, 0, s>>>(obj, view, A.batch, p, a);
-    CNO_CUDA(cudaGetLastError());
-    return CNO_OK;
-  }
-  int inner(const cno_stop_t& stop) {
-    const cno::AugLagFn<Obj> composite{obj, view};
-    cno_batch_out_t inner_out{};
-    inner_out.x = a.x_work;
-    inner_out.nfev = const_cast<uint32_t*>(a.inner_nfev);
-    cno_launch_info_t inner_info{};
-    const LaunchArgs la{A.objective, A.batch, a.x, &stop, &inner_out, queue, s, &inner_info};
-    return lbfgs(composite, la);
-  }
-  int outer_step(int* remaining) {
-    CNO_CUDA(cudaMemsetAsync(a.remaining, 0, sizeof(int), s));
-    cno::al_outer_step_kernel<Obj><<<blocks, threads, 0, s>>>(obj, view, A.batch, p, a);
-    CNO_CUDA(cudaGetLastError());
-    CNO_CUDA(cudaMemcpyAsync(remaining, a.remaining, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CNO_CUDA(cudaStreamSynchronize(s));
-    return CNO_OK;
-  }
-  int finalize() {
-    cno::al_finalize_kernel<T, Obj::Dim><<<blocks, threads, 0, s>>>(A.batch, view.n_eq, view.n_ineq, a);
-    CNO_CUDA(cudaGetLastError());
-    return CNO_OK;
-  }
-};
-
-template <class Obj>
-int al_run(const Obj& obj, const AlArgs& A) {
-  using T = typename Obj::Scalar;
-  constexpr int D = Obj::Dim;
-  const int ne = A.constraints->n_eq, ni = A.constraints->n_ineq;
-  const AlLayout L((size_t)A.batch, D, (size_t)ne, (size_t)ni, sizeof(T));
-  AlCudaBackend<Obj> be{obj, A, cno::al_make_arrays<T>(*A.out, A.workspace, L), {}, {}, A.workspace + L.queue, A.stream,
-                        (int)((A.batch + cno::kAlWarps - 1) / cno::kAlWarps), cno::kAlWarps * 32};
-  be.view = cno::al_make_view<T>(*A.constraints, be.a);
-  be.p = cno::al_make_params<T>(*A.config, *A.outer_stop);
-  int launches = 0;
-  const int rc = cno::al_outer_loop<T>(be, be.a, A.batch, D, ne, ni, A.x0, A.eq0, A.ineq0, A.penalty0, *A.inner_stop,
-                                       *A.config, &launches);
-  if (rc) return rc;
-  if (A.info) A.info->kernel_launches = launches;
-  return CNO_OK;
+int al_rows(const Obj& obj, const cno_constraints_t* k, const cno::AlArgs& a) {
+  return cno::al_run(obj, cno::AlRows{}, *k, a, g_last_cuda);
 }
-
 template <class T, int D>
-int al_rosenbrock(const AlArgs& a) { return al_run(cno::RosenbrockFn<T, D>{}, a); }
+int al_rosenbrock(const cno_problem_t*, const cno_constraints_t* k, const cno::AlArgs& a) {
+  return al_rows(cno::RosenbrockFn<T, D>{}, k, a);
+}
 template <class T, int D>
-int al_half_sq_norm(const AlArgs& a) { return al_run(cno::HalfSquaredNormFn<T, D>{}, a); }
+int al_half_sq_norm(const cno_problem_t*, const cno_constraints_t* k, const cno::AlArgs& a) {
+  return al_rows(cno::HalfSquaredNormFn<T, D>{}, k, a);
+}
 template <class T, int D>
-int al_dense_quadratic(const AlArgs& a) {  // the batched "QP with affine / ball constraints"
-  const cno_problem_t* p = a.objective;
+int al_dense_quadratic(const cno_problem_t* p, const cno_constraints_t* k, const cno::AlArgs& a) {
+  // the batched "QP with affine / ball constraints"
   if (!data_block_ok<T>(p, (int64_t)D * D + D, false)) return CNO_ERR_INVALID_ARGUMENT;
-  return al_run(cno::DenseQuadraticGlobalFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, a);
+  return al_rows(cno::DenseQuadraticGlobalFn<T, D>{static_cast<const T*>(p->data), (long long)p->data_stride}, k, a);
 }
 
 struct AlEntry {
   int family, dtype, d;
-  int (*fn)(const AlArgs&);
+  int (*fn)(const cno_problem_t*, const cno_constraints_t*, const cno::AlArgs&);
 };
 const AlEntry kAlTable[] = {
     {CNO_FN_ROSENBROCK, CNO_F64, 2, al_rosenbrock<double, 2>},
@@ -1225,8 +1144,8 @@ int cno_al_workspace_bytes(const cno_problem_t* objective, const cno_constraints
   if (rc) return rc;
   if (!bytes || batch < 0) return CNO_ERR_INVALID_ARGUMENT;
   const size_t ts = objective->dtype == CNO_F64 ? 8 : 4;
-  *bytes = AlLayout((size_t)batch, (size_t)objective->d, (size_t)constraints->n_eq,
-                    (size_t)constraints->n_ineq, ts).total;
+  *bytes = cno::AlLayout((size_t)batch, (size_t)objective->d, (size_t)constraints->n_eq,
+                         (size_t)constraints->n_ineq, ts).total;
   return CNO_OK;
 }
 
@@ -1241,31 +1160,16 @@ int cno_al_minimize(const cno_problem_t* objective, const cno_constraints_t* con
   if (batch < 0 || !out) return CNO_ERR_INVALID_ARGUMENT;
   if (info) memset(info, 0, sizeof(*info));
   if (batch == 0) return have_device() ? CNO_OK : CNO_ERR_NO_DEVICE;
-  if (!x0 || !out->x || !out->penalty || !out->max_violation || !out->max_lagrangian_gradient ||
-      !out->num_iterations || !out->status || !out->nfev)
-    return CNO_ERR_INVALID_ARGUMENT;  // they are the solver's state between outer iterations
-  if ((constraints->n_eq > 0 && !out->equality_multipliers) ||
-      (constraints->n_ineq > 0 && !out->inequality_multipliers))
-    return CNO_ERR_INVALID_ARGUMENT;
-  if (((uintptr_t)x0 & 15) || ((uintptr_t)out->x & 15)) return CNO_ERR_INVALID_ARGUMENT;
-  const size_t ts = objective->dtype == CNO_F64 ? 8 : 4;
-  const AlLayout L((size_t)batch, (size_t)objective->d, (size_t)constraints->n_eq,
-                   (size_t)constraints->n_ineq, ts);
-  if (!workspace || workspace_bytes < L.total || ((uintptr_t)workspace & 255)) return CNO_ERR_WORKSPACE;
+  cno::AlArgs a{(long long)batch, x0, eq0, ineq0, penalty0, inner_stop, outer_stop, config, out,
+                static_cast<unsigned char*>(workspace), workspace_bytes, static_cast<cudaStream_t>(stream), info};
   cno_stop_t idflt;
-  if ((rc = resolve_stop(inner_stop, &idflt, cno_default_stop))) return rc;
   cno_al_stop_t odflt;
-  if (!outer_stop) { cno_al_default_stop(&odflt); outer_stop = &odflt; }
   cno_al_config_t cdflt;
-  if (!config) { cno_al_default_config(&cdflt); config = &cdflt; }
+  if ((rc = cno::al_check_args(a, (size_t)objective->d, constraints->n_eq, constraints->n_ineq,
+                               objective->dtype == CNO_F64 ? 8 : 4, &idflt, &odflt, &cdflt)))
+    return rc;
   if (!have_device()) return CNO_ERR_NO_DEVICE;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cno::LaunchTimer timer(s, info);
-  if ((rc = timer.start(g_last_cuda))) return rc;
-  const AlArgs a{objective, constraints, (long long)batch, x0, eq0, ineq0, penalty0, inner_stop,
-                 outer_stop, config, out, static_cast<unsigned char*>(workspace), s, info};
-  if ((rc = al_find(objective)->fn(a))) return rc;
-  return timer.stop(g_last_cuda);
+  return al_find(objective)->fn(objective, constraints, a);
 }
 
 }  // extern "C"

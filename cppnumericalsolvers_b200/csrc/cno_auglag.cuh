@@ -15,11 +15,18 @@
 //   solver/progress.h:162-252              Progress::Update, constrained branch
 //
 // One outer iteration on the device = [al_autoscale_kernel on the first] ->
-// lbfgs_minimize_kernel<AugLagFn<Obj>> (the inner solve, skipping finished instances
+// lbfgs_minimize_kernel<AugLagFn<Obj, Cons>> (the inner solve, skipping finished instances
 // through AugLagFn::active) -> al_outer_step_kernel.  Everything per-instance lives in
 // [B, .] arrays in HBM between launches; inside a launch it is registers only.
+//
+// Cons, the constraint set, is the only place a constraint is evaluated:
+//   AlRows (the default)       the [a | t] rows of AlView (cno_constraints_t, cno_al_minimize)
+//   AlFunctors<EqList, InList> two compile-time lists of device functors (function_problem.h:54-107 with
+//                              FunctionExpr constraints; cno_<tag>_al_minimize, include/cppoptlib_b200/device.cuh)
 #ifndef CNO_AUGLAG_CUH_
 #define CNO_AUGLAG_CUH_
+
+#include <type_traits>
 
 #include "../../include/cno_al.h"
 #include "cno_device.cuh"
@@ -62,16 +69,74 @@ __device__ __forceinline__ T al_con_eval(const AlView<T>& v, long long instance,
   return t - warp_sum(lane_dot<T, E>(x, x));
 }
 
-// ToAugmentedLagrangian(prob, multipliers, penalty) as a First-mode device functor.
-template <class Obj>
-struct AugLagFn {
+// The row constraint set: constraint idx is row idx of the instance (al_con_eval).
+struct AlRows {
+  template <class T, int D>
+  __device__ __forceinline__ T eval(const AlView<T>& v, const EvalCtx& c, int idx, const T (&x)[Shape<D>::E],
+                                    T (&gc)[Shape<D>::E]) const {
+    return al_con_eval<T, D>(v, c.instance, idx, c.lane, x, gc);
+  }
+};
+
+// Constraint i of a functor list (members head, tail; static size), picked by a warp-uniform index: an if-chain
+// over the list, so the callers' loops over constraints stay one loop.
+template <class T, int E, class L>
+__device__ __forceinline__ T al_list_eval(const L& l, const EvalCtx& c, int i, const T (&x)[E], T (&gc)[E]) {
+  if constexpr (L::size == 0) {
+    return T(0);  // (never reached: i < the list's size)
+  } else {
+    if (uni(i == 0)) return l.head(c, x, &gc);
+    return al_list_eval<T, E>(l.tail, c, i - 1, x, gc);
+  }
+}
+
+// Every functor of a list follows the device concept with the objective's Scalar and Dim.
+template <class T, int D, class L, bool kEmpty = (L::size == 0)>
+struct AlListOk {
+  using H = decltype(L::head);
+  static constexpr bool value = std::is_same<typename H::Scalar, T>::value && H::Dim == D && H::Mode >= 1 &&
+                                AlListOk<T, D, decltype(L::tail)>::value;
+};
+template <class T, int D, class L>
+struct AlListOk<T, D, L, true> : std::true_type {};
+
+// The functor constraint set: equalities c(x) == 0, then inequalities c(x) >= 0 (function_problem.h:54-107).  A
+// Second-mode functor is used as a First-mode one (function_base.h:210-230): only operator() is called.
+template <class EqList, class IneqList>
+struct AlFunctors {
+  static constexpr int kNumEq = EqList::size;
+  static constexpr int kNumIneq = IneqList::size;
+  static_assert(kNumEq <= kAlMaxCon && kNumIneq <= kAlMaxCon, "at most kAlMaxCon (32) constraints of each kind");
+  EqList eq;
+  IneqList ineq;
+  template <class T, int D>
+  __device__ __forceinline__ T eval(const AlView<T>&, const EvalCtx& c, int idx, const T (&x)[Shape<D>::E],
+                                    T (&gc)[Shape<D>::E]) const {
+    static_assert(AlListOk<T, D, EqList>::value && AlListOk<T, D, IneqList>::value,
+                  "constraint functors: the objective's Scalar and Dim, Mode >= 1");
+    if (uni(idx < kNumEq)) return al_list_eval<T, Shape<D>::E>(eq, c, idx, x, gc);
+    return al_list_eval<T, Shape<D>::E>(ineq, c, idx - kNumEq, x, gc);
+  }
+};
+
+// ToAugmentedLagrangian(prob, multipliers, penalty) as a First-mode device functor.  The constraint set is a base
+// so that the empty AlRows adds no bytes: the built-in path keeps its layout and code.
+template <class Obj, class Cons = AlRows>
+struct AugLagFn : Cons {
   using Scalar = typename Obj::Scalar;
   static constexpr int Dim = Obj::Dim;
   static constexpr int Mode = 1;
   static constexpr int E = Shape<Dim>::E;
   using T = Scalar;
+  static_assert(Dim <= 128, "AugmentedLagrangian: d <= 128");
   Obj obj;
   AlView<T> v;
+
+  __host__ __device__ __forceinline__ AugLagFn(const Obj& o, const AlView<T>& view, const Cons& cons = Cons{})
+      : Cons(cons), obj(o), v(view) {}
+  __device__ __forceinline__ T con(const EvalCtx& c, int idx, const T (&x)[E], T (&gc)[E]) const {
+    return Cons::template eval<T, Dim>(v, c, idx, x, gc);
+  }
 
   // lbfgs_minimize_kernel skips instances whose outer loop has finished
   __device__ __forceinline__ bool active(long long b) const {
@@ -103,7 +168,7 @@ struct AugLagFn {
 #pragma unroll
         for (int k = 0; k < E; ++k) gc[k] = T(0);
       } else {
-        const T cv = al_con_eval<T, Dim>(v, c.instance, i, c.lane, x, gc);
+        const T cv = con(c, i, x, gc);
         tv = l * cv;
 #pragma unroll
         for (int k = 0; k < E; ++k) gc[k] = l * gc[k];
@@ -124,7 +189,7 @@ struct AugLagFn {
 #pragma unroll
         for (int k = 0; k < E; ++k) gc[k] = T(0);
       } else {
-        const T cv = al_con_eval<T, Dim>(v, c.instance, i, c.lane, x, gc);
+        const T cv = con(c, i, x, gc);
         const T pv = cv * cv;  // Prod: (f g, g * grad_f + f * grad_g)
 #pragma unroll
         for (int k = 0; k < E; ++k) gc[k] = cv * gc[k] + cv * gc[k];
@@ -149,7 +214,7 @@ struct AugLagFn {
 #pragma unroll 1
       for (int j = 0; j < v.n_ineq; ++j) {
         const T m = mu[j];
-        const T gv = al_con_eval<T, Dim>(v, c.instance, v.n_eq + j, c.lane, x, gc);
+        const T gv = con(c, v.n_eq + j, x, gc);
         T av = m - rho * gv;  // argument = Const(mu) - rho * g
 #pragma unroll
         for (int k = 0; k < E; ++k) gc[k] = T(0) - rho * gc[k];
@@ -251,10 +316,10 @@ __device__ __forceinline__ void al_store(T* row, int lane, const T (&v)[Shape<D>
 constexpr int kAlWarps = 8;
 
 // ComputeAutoScaledPenalty (augmented_lagrangian.h:312-318, 451-476) on outer iteration 1.
-template <class Obj>
+template <class Obj, class Cons = AlRows>
 __global__ void __launch_bounds__(kAlWarps * 32)
 al_autoscale_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const long long batch,
-                    const AlParams<typename Obj::Scalar> p, AlArrays<typename Obj::Scalar> a) {
+                    const AlParams<typename Obj::Scalar> p, AlArrays<typename Obj::Scalar> a, const Cons cons = Cons{}) {
   using T = typename Obj::Scalar;
   constexpr int D = Obj::Dim;
   constexpr int E = Shape<D>::E;
@@ -270,12 +335,12 @@ al_autoscale_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const l
   T srs = T(0);
 #pragma unroll 1
   for (int i = 0; i < v.n_eq; ++i) {
-    const T c = al_con_eval<T, D>(v, b, i, lane, x, gc);
+    const T c = cons.template eval<T, D>(v, ctx, i, x, gc);
     srs += T(0.5) * c * c;
   }
 #pragma unroll 1
   for (int j = 0; j < v.n_ineq; ++j) {
-    const T c = al_con_eval<T, D>(v, b, v.n_eq + j, lane, x, gc);
+    const T c = cons.template eval<T, D>(v, ctx, v.n_eq + j, x, gc);
     if (uni(c < T(0))) srs += T(0.5) * c * c;
   }
   const T denom = smax(srs, T(1));
@@ -288,10 +353,10 @@ al_autoscale_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const l
 
 // The rest of OptimizationStep after the inner solve (augmented_lagrangian.h:356-433) and
 // Progress::Update's constrained branch (progress.h:162-252).
-template <class Obj>
+template <class Obj, class Cons = AlRows>
 __global__ void __launch_bounds__(kAlWarps * 32)
 al_outer_step_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const long long batch,
-                     const AlParams<typename Obj::Scalar> p, AlArrays<typename Obj::Scalar> a) {
+                     const AlParams<typename Obj::Scalar> p, AlArrays<typename Obj::Scalar> a, const Cons cons = Cons{}) {
   using T = typename Obj::Scalar;
   constexpr int D = Obj::Dim;
   constexpr int E = Shape<D>::E;
@@ -305,7 +370,7 @@ al_outer_step_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const 
     if (!((s == CNO_STATUS_CONTINUE) | (s == CNO_STATUS_NOT_STARTED))) return;
   }
   const EvalCtx ctx{lane, b, nullptr};
-  const AugLagFn<Obj> composite{obj, v};
+  const AugLagFn<Obj, Cons> composite(obj, v, cons);
   T* const lam = a.lambda + b * v.n_eq;
   T* const mu = a.mu + b * v.n_ineq;
   T* const prev_lam = prev_mult[warp];
@@ -325,7 +390,7 @@ al_outer_step_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const 
   T max_violation = T(0);
 #pragma unroll 1
   for (int i = 0; i < v.n_eq; ++i) {
-    const T cv = al_con_eval<T, D>(v, b, i, lane, x, gc);
+    const T cv = composite.con(ctx, i, x, gc);
     max_violation = smax(max_violation, cabs(cv));
     if (lane == i) {
       const T cand = my_lam + penalty * cv;
@@ -334,7 +399,7 @@ al_outer_step_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const 
   }
 #pragma unroll 1
   for (int j = 0; j < v.n_ineq; ++j) {
-    const T cv = al_con_eval<T, D>(v, b, v.n_eq + j, lane, x, gc);
+    const T cv = composite.con(ctx, v.n_eq + j, x, gc);
     const T violation = smax(T(0), -cv);
     max_violation = smax(max_violation, violation);
     if (lane == j) {
@@ -351,14 +416,14 @@ al_outer_step_kernel(const Obj obj, const AlView<typename Obj::Scalar> v, const 
   const T objective = obj(ctx, x, &sum_grad);
 #pragma unroll 1
   for (int i = 0; i < v.n_eq; ++i) {
-    al_con_eval<T, D>(v, b, i, lane, x, gc);
+    composite.con(ctx, i, x, gc);
     const T l = __shfl_sync(kFullMask, my_lam, i);
 #pragma unroll
     for (int k = 0; k < E; ++k) sum_grad[k] = sum_grad[k] + l * gc[k];
   }
 #pragma unroll 1
   for (int j = 0; j < v.n_ineq; ++j) {
-    al_con_eval<T, D>(v, b, v.n_eq + j, lane, x, gc);
+    composite.con(ctx, v.n_eq + j, x, gc);
     const T m = __shfl_sync(kFullMask, my_mu, j);
 #pragma unroll
     for (int k = 0; k < E; ++k) sum_grad[k] = sum_grad[k] - m * gc[k];

@@ -1,13 +1,14 @@
 // cno_auglag_host.h -- the host side of AugmentedLagrangian::Minimize (solver/augmented_lagrangian.h:
 // 295-449), independent of how memory is moved and kernels are launched: the outer loop, the scratch
-// layout, the parameter narrowing.  csrc/cno_api.cu drives it with the CUDA backend; tests/emu drives
-// the SAME code with the CPU warp emulation (the `-m "not gpu"` check of this logic; DESIGN.md 8).
+// layout, the parameter narrowing.  csrc/cno_auglag_launch.cuh drives it with the CUDA backend (for cno_al_minimize and
+// cno_<tag>_al_minimize); tests/emu drives the SAME code with the CPU warp emulation (the `-m "not gpu"` check of this
+// logic; DESIGN.md 8).
 //
 // Backend concept (all return 0 or a cno_error_t):
 //   int copy_or_zero(void* dst, const void* src, size_t bytes)   device copy, or zero fill when src == nullptr
 //   int fill(void* dst, int byte, size_t bytes)
 //   int autoscale()                                              al_autoscale_kernel
-//   int inner(const cno_stop_t& stop)                            lbfgs_minimize_kernel<AugLagFn<Obj>>: x -> x_work, inner_nfev
+//   int inner(const cno_stop_t& stop)                            lbfgs_minimize_kernel<AugLagFn<Obj, Cons>>: x -> x_work, inner_nfev
 //   int outer_step(int* remaining)                               al_outer_step_kernel; instances still running
 //   int finalize()                                               al_finalize_kernel
 #ifndef CNO_AUGLAG_HOST_H_

@@ -44,6 +44,7 @@
 
 #include "../cno.h"
 #include "../cno_al.h"
+#include "constraint_list.h"
 #include "modes.h"
 
 namespace cppoptlib {
@@ -814,7 +815,7 @@ namespace function {
 // a constraint is a row [a (d) | t]; AFFINE c(x) = a.x - t, SQNORM c(x) = t - x.x; equalities
 // (c == 0) first, then inequalities (c >= 0).  `rows` is one set shared by the batch
 // ([n_con][d+1]) or per instance ([B][n_con][d+1]).
-template <class Objective>
+template <class Objective, class EqualityList = void, class InequalityList = void>
 struct ConstrainedOptimizationProblem {
   using ScalarType = typename Objective::ScalarType;
   static constexpr int Dimension = Objective::Dimension;
@@ -826,6 +827,38 @@ struct ConstrainedOptimizationProblem {
   bool per_instance = false;
   int n_ineq() const { return static_cast<int>(kinds.size()) - n_eq; }
 };
+
+// function_problem.h:54-107 with functor constraints: any user functor or composite (expressions.h) of the
+// objective's scalar type and dimension, Second-mode ones used as First mode.  Equalities (c == 0) then
+// inequalities (c >= 0), at most 32 of each.  A trivially copyable value: the AL kernels take it by value.
+//   using P = ConstrainedOptimizationProblem<NegProduct, Equalities<>, Inequalities<Ellipse>>;
+//   CNO_DECLARE_CONSTRAINED(hs029, P)      host side: binds P to the symbols
+//   CNO_INSTANTIATE_CONSTRAINED(hs029, P)  nvcc translation unit: defines them (device.cuh)
+template <class Objective, class... Eq, class... Ineq>
+struct ConstrainedOptimizationProblem<Objective, Equalities<Eq...>, Inequalities<Ineq...>> {
+  using ScalarType = typename Objective::ScalarType;
+  static constexpr int Dimension = Objective::Dimension;
+  static constexpr DifferentiabilityMode Differentiability = Objective::Differentiability;
+  static constexpr int kNumEq = static_cast<int>(sizeof...(Eq));
+  static constexpr int kNumIneq = static_cast<int>(sizeof...(Ineq));
+  static_assert(kNumEq <= 32 && kNumIneq <= 32, "at most 32 equality and 32 inequality constraints");
+  static_assert(Dimension >= 1 && Dimension <= 128, "AugmentedLagrangian: 1 <= d <= 128");
+  static_assert(((std::is_same_v<typename Eq::ScalarType, ScalarType> && Eq::Dimension == Dimension) && ...) &&
+                    ((std::is_same_v<typename Ineq::ScalarType, ScalarType> && Ineq::Dimension == Dimension) && ...),
+                "constraints must have the objective's scalar type and dimension");
+  Objective objective;
+  Equalities<Eq...> equality_constraints;
+  Inequalities<Ineq...> inequality_constraints;
+};
+
+// The cno_<tag>_al_* symbols of a functor-constrained problem (specialised by CNO_DECLARE_CONSTRAINED).
+typedef int (*RawAlWorkspaceBytesFn)(int64_t batch, size_t* bytes);
+typedef int (*RawAlMinimizeFn)(const void* problem_bytes, int64_t batch, const void* x0, const void* eq0,
+                               const void* ineq0, const void* penalty0, const cno_stop_t* inner_stop,
+                               const cno_al_stop_t* outer_stop, const cno_al_config_t* config, const cno_al_out_t* out,
+                               void* workspace, size_t workspace_bytes, void* stream, cno_launch_info_t* info);
+template <class P>
+struct ConstrainedLauncherTraits;
 }  // namespace function
 
 namespace solver {
@@ -865,9 +898,28 @@ struct BatchedAugmentedLagrangeState {
   }
 };
 
-// AugmentedLagrangian<Problem, Lbfgs<...>> (solver/augmented_lagrangian.h:278-449).
+namespace al_detail {
+template <class P>
+struct IsFunctorConstrained : std::false_type {};
+template <class O, class... Eq, class... Ineq>
+struct IsFunctorConstrained<
+    function::ConstrainedOptimizationProblem<O, function::Equalities<Eq...>, function::Inequalities<Ineq...>>>
+    : std::true_type {};
+template <class S>
+struct IsDefaultLbfgs : std::false_type {};
+template <class F>
+struct IsDefaultLbfgs<Lbfgs<F, 10, linesearch::MoreThuente>> : std::true_type {};
+}  // namespace al_detail
+
+// AugmentedLagrangian<Problem, Lbfgs<...>> (solver/augmented_lagrangian.h:278-449).  On a problem with functor
+// constraints it runs the symbols of CNO_DECLARE_CONSTRAINED(tag, Problem); their inner kernel is
+// Lbfgs<composite, 10, MoreThuente>.
 template <class ProblemType, class solver_t>
 class AugmentedLagrangian {
+  static constexpr bool kFunctorConstraints = al_detail::IsFunctorConstrained<ProblemType>::value;
+  static_assert(!kFunctorConstraints || al_detail::IsDefaultLbfgs<solver_t>::value,
+                "AugmentedLagrangian on functor constraints: the inner solver is Lbfgs<F, 10, MoreThuente>");
+
  public:
   using ScalarType = typename ProblemType::ScalarType;
   using StateType = BatchedAugmentedLagrangeState<ScalarType, ProblemType::Dimension>;
@@ -886,17 +938,14 @@ class AugmentedLagrangian {
     using T = ScalarType;
     constexpr int D = ProblemType::Dimension;
     const int64_t B = state.batch;
-    const int ne = problem_.n_eq, ni = problem_.n_ineq();
-    function::FunctionExpr<T, ProblemType::Differentiability, D> expr(problem_.objective);
-    if (expr.raw) throw std::runtime_error("AugmentedLagrangian: built-in objective families only");
-    auto kinds = detail::DeviceArray<int32_t>::FromHost(problem_.kinds);
-    auto rows = detail::DeviceArray<T>::FromHost(problem_.rows);
-    cno_constraints_t k{};
-    k.n_eq = ne;
-    k.n_ineq = ni;
-    k.kinds = kinds.data();
-    k.data = rows.data();
-    k.data_stride = problem_.per_instance ? static_cast<int64_t>(problem_.kinds.size()) * (D + 1) : 0;
+    int ne, ni;
+    if constexpr (kFunctorConstraints) {
+      ne = ProblemType::kNumEq;
+      ni = ProblemType::kNumIneq;
+    } else {
+      ne = problem_.n_eq;
+      ni = problem_.n_ineq();
+    }
 
     StateType result;
     result.batch = B;
@@ -928,9 +977,6 @@ class AugmentedLagrangian {
     out.f_delta = prog.f_delta.data();
     out.gradient_norm = prog.gradient_norm.data();
 
-    size_t nbytes = 0;
-    detail::check_cno(cno_al_workspace_bytes(&expr.problem, &k, B, &nbytes), "cno_al_workspace_bytes");
-    detail::DeviceArray<unsigned char> workspace(nbytes < 256 ? 256 : nbytes);
     const cno_stop_t inner = unconstrained_solver_template_.stopping_progress.to_c();
     cno_al_stop_t outer{};
     outer.num_iterations = stopping_progress.num_iterations;
@@ -947,12 +993,33 @@ class AugmentedLagrangian {
     cfg.warmup_inner_gradient_tolerance = config_.warmup_inner_gradient_tolerance;
     cfg.multiplier_max = config_.multiplier_max;
     cfg.kkt_gradient_tolerance = config_.kkt_gradient_tolerance;
-    detail::check_cno(
-        cno_al_minimize(&expr.problem, &k, B, state.x.data(),
-                        ne ? state.equality_multipliers.data() : nullptr,
-                        ni ? state.inequality_multipliers.data() : nullptr, state.penalty.data(), &inner, &outer, &cfg,
-                        &out, workspace.data(), workspace.size(), stream, &prog.launch),
-        "cno_al_minimize");
+    const void* eq0 = ne ? state.equality_multipliers.data() : nullptr;
+    const void* ineq0 = ni ? state.inequality_multipliers.data() : nullptr;
+    size_t nbytes = 0;
+    if constexpr (kFunctorConstraints) {  // the symbols of CNO_DECLARE_CONSTRAINED(tag, ProblemType)
+      using L = function::ConstrainedLauncherTraits<ProblemType>;
+      detail::check_cno(L::workspace_bytes(B, &nbytes), "cno_<tag>_al_workspace_bytes");
+      detail::DeviceArray<unsigned char> workspace(nbytes < 256 ? 256 : nbytes);
+      detail::check_cno(L::minimize(&problem_, B, state.x.data(), eq0, ineq0, state.penalty.data(), &inner, &outer, &cfg,
+                                    &out, workspace.data(), workspace.size(), stream, &prog.launch),
+                        "cno_<tag>_al_minimize");
+    } else {
+      function::FunctionExpr<T, ProblemType::Differentiability, D> expr(problem_.objective);
+      if (expr.raw) throw std::runtime_error("AugmentedLagrangian: built-in objective families only");
+      auto kinds = detail::DeviceArray<int32_t>::FromHost(problem_.kinds);
+      auto rows = detail::DeviceArray<T>::FromHost(problem_.rows);
+      cno_constraints_t k{};
+      k.n_eq = ne;
+      k.n_ineq = ni;
+      k.kinds = kinds.data();
+      k.data = rows.data();
+      k.data_stride = problem_.per_instance ? static_cast<int64_t>(problem_.kinds.size()) * (D + 1) : 0;
+      detail::check_cno(cno_al_workspace_bytes(&expr.problem, &k, B, &nbytes), "cno_al_workspace_bytes");
+      detail::DeviceArray<unsigned char> workspace(nbytes < 256 ? 256 : nbytes);
+      detail::check_cno(cno_al_minimize(&expr.problem, &k, B, state.x.data(), eq0, ineq0, state.penalty.data(), &inner,
+                                        &outer, &cfg, &out, workspace.data(), workspace.size(), stream, &prog.launch),
+                        "cno_al_minimize");
+    }
     return {std::move(result), std::move(prog)};
   }
 
@@ -998,6 +1065,24 @@ class AugmentedLagrangian {
       e.pod.assign(reinterpret_cast<const unsigned char*>(&f),                                                   \
                    reinterpret_cast<const unsigned char*>(&f) + sizeof(F));                                      \
     }                                                                                                             \
+  };                                                                                                              \
+  }
+
+// Declares (for a host translation unit) the extern "C" launchers that CNO_INSTANTIATE_CONSTRAINED(tag, P) defines
+// in an nvcc translation unit, and binds the functor-constrained problem P to them.
+#define CNO_DECLARE_CONSTRAINED(tag, P)                                                                          \
+  extern "C" int cno_##tag##_al_workspace_bytes(int64_t batch, size_t* bytes);                                    \
+  extern "C" int cno_##tag##_al_minimize(const void* problem_bytes, int64_t batch, const void* x0, const void* eq0, \
+                                         const void* ineq0, const void* penalty0, const cno_stop_t* inner_stop,   \
+                                         const cno_al_stop_t* outer_stop, const cno_al_config_t* config,          \
+                                         const cno_al_out_t* out, void* workspace, size_t workspace_bytes,        \
+                                         void* stream, cno_launch_info_t* info);                                  \
+  namespace cppoptlib::function {                                                                                 \
+  template <>                                                                                                     \
+  struct ConstrainedLauncherTraits<P> {                                                                           \
+    static_assert(std::is_trivially_copyable_v<P>, "the problem is passed to the kernels by value");            \
+    static constexpr RawAlWorkspaceBytesFn workspace_bytes = &cno_##tag##_al_workspace_bytes;                    \
+    static constexpr RawAlMinimizeFn minimize = &cno_##tag##_al_minimize;                                        \
   };                                                                                                              \
   }
 

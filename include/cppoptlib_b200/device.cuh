@@ -25,6 +25,15 @@
 //   cno_<tag>_minimize_steps  OptimizationStep rounds + callback  (solver.h:163-176, 226-228; Lbfgs)
 //   cno_<tag>_evaluate        F::operator()(x, &grad) per instance (function_base.h:103-120)
 //   cno_<tag>_condition_hessian   Progress::condition_hessian at x per instance (progress.h:203-210; Second mode)
+//
+// A constrained problem with functor constraints (cppoptlib.h: ConstrainedOptimizationProblem<Objective,
+// Equalities<C...>, Inequalities<C...>>; objective and constraints any functors or composites of one Scalar and
+// Dim <= 128):
+//   CNO_DECLARE_CONSTRAINED(tag, P)       host side (cppoptlib.h)
+//   CNO_INSTANTIATE_CONSTRAINED(tag, P)   device side: defines
+//   cno_<tag>_al_workspace_bytes / cno_<tag>_al_minimize   AugmentedLagrangian<P, Lbfgs>::Minimize
+//        (augmented_lagrangian.h:278-449), with the contract of cno_al_minimize (include/cno_al.h) and its kernels,
+//        the constraint set being P's functors instead of [a | t] rows
 #ifndef CPPOPTLIB_B200_DEVICE_CUH_
 #define CPPOPTLIB_B200_DEVICE_CUH_
 
@@ -36,6 +45,7 @@
 #define CPPOPTLIB_B200_WITH_DEVICE 1
 #include "cppoptlib.h"
 #include "expressions.h"
+#include "cno_auglag_launch.cuh"
 #include "cno_bfgs.cuh"
 #include "cno_descent.cuh"
 #include "cno_evaluate.cuh"
@@ -205,7 +215,57 @@ inline int user_state_bytes(int solver, int64_t batch, size_t* bytes) {
   *bytes = (size_t)batch * RL::kBytes;
   return CNO_OK;
 }
+// AugmentedLagrangian<P, Lbfgs>::Minimize for a functor-constrained problem P: cno_al_minimize's checks, workspace
+// layout and kernels, with AlFunctors over P's lists as the constraint set.
+template <class P>
+inline int user_al_workspace_bytes(int64_t batch, size_t* bytes) {
+  if (!bytes || batch < 0) return CNO_ERR_INVALID_ARGUMENT;
+  *bytes = AlLayout((size_t)batch, P::Dimension, P::kNumEq, P::kNumIneq, sizeof(typename P::ScalarType)).total;
+  return CNO_OK;
+}
+template <class P>
+inline int user_al_minimize(const P& prob, int64_t batch, const void* x0, const void* eq0, const void* ineq0,
+                            const void* penalty0, const cno_stop_t* inner_stop, const cno_al_stop_t* outer_stop,
+                            const cno_al_config_t* config, const cno_al_out_t* out, void* workspace,
+                            size_t workspace_bytes, void* stream, cno_launch_info_t* info) {
+  using Cons = AlFunctors<decltype(prob.equality_constraints), decltype(prob.inequality_constraints)>;
+  if (batch < 0 || !out) return CNO_ERR_INVALID_ARGUMENT;
+  if (info) *info = cno_launch_info_t{};
+  if (batch == 0) return CNO_OK;
+  AlArgs a{(long long)batch, x0, eq0, ineq0, penalty0, inner_stop, outer_stop, config, out,
+           static_cast<unsigned char*>(workspace), workspace_bytes, static_cast<cudaStream_t>(stream), info};
+  cno_stop_t idflt;
+  cno_al_stop_t odflt;
+  cno_al_config_t cdflt;
+  int rc = al_check_args(a, P::Dimension, Cons::kNumEq, Cons::kNumIneq, sizeof(typename P::ScalarType), &idflt, &odflt,
+                         &cdflt);
+  if (rc) return rc;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return CNO_ERR_NO_DEVICE;
+  cudaError_t last_error = cudaSuccess;
+  const cno_constraints_t k{Cons::kNumEq, Cons::kNumIneq, nullptr, nullptr, 0};
+  return al_run(prob.objective, Cons{prob.equality_constraints, prob.inequality_constraints}, k, a, last_error);
+}
 }  // namespace cno
+
+// CNO_INSTANTIATE_CONSTRAINED(tag, P): the AugmentedLagrangian symbols of a functor-constrained problem P.
+#define CNO_INSTANTIATE_CONSTRAINED(tag, P)                                                                    \
+  static_assert(std::is_trivially_copyable<P>::value, "the problem is passed to the kernels by value");       \
+  extern "C" int cno_##tag##_al_workspace_bytes(int64_t batch, size_t* bytes) {                                \
+    return cno::user_al_workspace_bytes<P>(batch, bytes);                                                      \
+  }                                                                                                            \
+  extern "C" int cno_##tag##_al_minimize(const void* problem_bytes, int64_t batch, const void* x0, const void* eq0, \
+                                         const void* ineq0, const void* penalty0, const cno_stop_t* inner_stop, \
+                                         const cno_al_stop_t* outer_stop, const cno_al_config_t* config,        \
+                                         const cno_al_out_t* out, void* workspace, size_t workspace_bytes,      \
+                                         void* stream, cno_launch_info_t* info) {                               \
+    if (!problem_bytes) return CNO_ERR_INVALID_ARGUMENT;                                                       \
+    alignas(P) unsigned char raw__[sizeof(P)];                                                                 \
+    memcpy(raw__, problem_bytes, sizeof(P));                                                                   \
+    return cno::user_al_minimize<P>(*reinterpret_cast<const P*>(raw__), batch, x0, eq0, ineq0, penalty0,       \
+                                    inner_stop, outer_stop, config, out, workspace, workspace_bytes, stream,   \
+                                    info);                                                                     \
+  }
 
 // CNO_INSTANTIATE_FUNCTION_M(tag, F, M): the same with the L-BFGS kernels compiled for Lbfgs<F, M> (lbfgs.h:40-41).
 #define CNO_INSTANTIATE_FUNCTION(tag, F) CNO_INSTANTIATE_FUNCTION_M(tag, F, CNO_LBFGS_M)
