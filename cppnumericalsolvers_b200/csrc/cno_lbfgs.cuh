@@ -28,6 +28,7 @@
 #include "cno_device.cuh"
 #include "cno_linesearch.cuh"
 #include "cno_kernel_params.h"
+#include "cno_progress.cuh"
 
 // Compile-time cap on the warps per CTA of every L-BFGS plan (default: none).  tools/lbfgs_warp_sweep.py builds
 // copies of the library with -DCNO_LBFGS_MAX_WARPS=w to measure throughput against resident warps.
@@ -76,92 +77,6 @@ struct YHist {
   __device__ __forceinline__ void wait(T (&)[E], Pending&) const {}
   __device__ __forceinline__ void fence_store() const {}
 };
-
-// progress.h:153-327 on warp-uniform scalars (FunctionState branch).  The
-// past-f ring (progress.h:138-140) lives in the warp's shared-memory slice.
-template <class T>
-struct ProgressState {
-  uint32_t num_iterations;
-  int x_delta_violations;
-  int f_delta_violations;
-  T x_delta, f_delta, gradient_norm;
-  int ring_size, ring_pos;
-  int status;
-};
-
-template <class T>
-__device__ __forceinline__ void progress_update(ProgressState<T>& p, const StopParams<T>& stop,
-                                                T* __restrict__ ring, const int lane,
-                                                T prev_value, T cur_value, T x_delta,
-                                                T gradient_norm, T x_inf) {
-  p.num_iterations++;
-  p.f_delta = cabs(cur_value - prev_value);
-  p.x_delta = x_delta;
-  p.gradient_norm = gradient_norm;
-  int status = CNO_STATUS_CONTINUE;
-  // Tests in the reference's order; the first that fires wins (each `return`
-  // of progress.h becomes "status already set").
-  if ((stop.num_iterations > 0) && ((unsigned long long)p.num_iterations > stop.num_iterations))
-    status = CNO_STATUS_ITERATION_LIMIT;  // :212-216
-  if (status == CNO_STATUS_CONTINUE) {    // :254-262
-    if ((stop.x_delta > 0) && (p.x_delta < stop.x_delta)) {
-      p.x_delta_violations++;
-      if (p.x_delta_violations >= stop.x_delta_violations) status = CNO_STATUS_X_DELTA_VIOLATION;
-    } else {
-      p.x_delta_violations = 0;
-    }
-  }
-  if (status == CNO_STATUS_CONTINUE) {  // :263-277
-    if ((stop.f_delta > 0) &&
-        (p.f_delta < stop.f_delta * (stop.f_delta_relative
-                                         ? smax(smax(cabs(cur_value), cabs(prev_value)), T(1))
-                                         : T(1)))) {
-      p.f_delta_violations++;
-      if (p.f_delta_violations >= stop.f_delta_violations) status = CNO_STATUS_F_DELTA_VIOLATION;
-    } else {
-      p.f_delta_violations = 0;
-    }
-  }
-  if (uni(status == CNO_STATUS_CONTINUE && stop.past > 0)) {  // :280-298
-    const int pp = stop.past;
-    if (uni(p.ring_size != pp)) {
-      if (lane < pp) ring[lane] = cur_value;
-      p.ring_size = pp;
-      p.ring_pos = 0;
-      __syncwarp();
-    }
-    bool fired = false;
-    if (uni((int)p.num_iterations > pp)) {
-      const T past_f = ring[p.ring_pos];
-      // rate = |past_f - f| / max(1, |f|) < past_delta (:287-290)?  A difference above twice (below half) the product
-      // past_delta * max(1, |f|) decides it without the division: the quotient is then above 2 (below 0.5) past_delta
-      // up to two roundings.  In between, or with a non-finite operand: the specification's expression.
-      const T diff = cabs(past_f - cur_value), mag = smax(T(1), cabs(cur_value));
-      const T bound = stop.past_delta * mag;
-      if (cfinite(diff) && cfinite(bound) && bound > T(0) && diff > T(2) * bound) {
-        fired = false;
-      } else if (cfinite(diff) && cfinite(bound) && bound >= Num<T>::min_normal && diff < T(0.5) * bound) {
-        fired = true;
-      } else {
-        const T rate = diff / mag;
-        fired = rate < stop.past_delta;
-      }
-    }
-    if (uni(fired)) {
-      status = CNO_STATUS_F_DELTA_VIOLATION;
-    } else {
-      __syncwarp();
-      if (lane == 0) ring[p.ring_pos] = cur_value;
-      p.ring_pos = (p.ring_pos + 1 == pp) ? 0 : p.ring_pos + 1;
-      __syncwarp();
-    }
-  }
-  if (status == CNO_STATUS_CONTINUE && stop.gradient_norm > 0) {  // :299-317
-    const T scale = stop.gradient_norm_relative ? smax(T(1), x_inf) : T(1);
-    if (p.gradient_norm < stop.gradient_norm * scale) status = CNO_STATUS_GRADIENT_NORM_VIOLATION;
-  }
-  p.status = status;
-}
 
 // Record of one parked instance (stepwise solves): S slots, Y slots (lane-major),
 // then scalars.  What Lbfgs keeps as members between OptimizationStep calls
@@ -270,9 +185,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
 
   for (; solver_warp;) {
     // ---- retire + refill: next instance from the global queue ----
-    unsigned long long b = 0;
-    if (lane == 0) b = atomicAdd(queue, 1ULL);
-    b = __shfl_sync(kFullMask, b, 0);
+    const unsigned long long b = claim_instance(queue, lane);
     if (uni(b >= (unsigned long long)batch)) break;
     if constexpr (FnSkipsInstances<Fn>::value) {  // e.g. AugLagFn: the instance's outer loop has finished
       if (uni(!fn.active((long long)b))) continue;
@@ -292,7 +205,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     T gamma;
     T xx;            // ||x||^2 carried across iterations (the dot the reference recomputes at lbfgs.h:95)
     ProgressState<T> prog;
-    prog.x_delta = prog.f_delta = prog.gradient_norm = T(0);
+    progress_start(prog);
     bool resumed = false;
     using RL = ResumeLayout<T, E, M>;
     if constexpr (kResume) {
@@ -343,12 +256,6 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       mem_pos = 0;
       valid = 0;
       gamma = T(1);
-      prog.num_iterations = 0;
-      prog.x_delta_violations = 0;
-      prog.f_delta_violations = 0;
-      prog.ring_size = 0;
-      prog.ring_pos = 0;
-      prog.status = CNO_STATUS_NOT_STARTED;
       xx = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(x, x), rc);
     }
     int local_it = 0;
@@ -684,19 +591,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       }
     }
 
-    // ---- write the returned FunctionState + Progress ----
-    if (out.x) store_row<T, D>(out.x + b * D, lane, x);
-    if (out.gradient) store_row<T, D>(out.gradient + b * D, lane, g);
-    if (lane == 0) {
-      if (out.value) out.value[b] = f;
-      if (out.num_iterations) out.num_iterations[b] = prog.num_iterations;
-      if (out.status) out.status[b] = (int8_t)prog.status;
-      if (out.nfev) out.nfev[b] = nfev;
-      if (out.x_delta) out.x_delta[b] = prog.x_delta;
-      if (out.f_delta) out.f_delta[b] = prog.f_delta;
-      if (out.gradient_norm) out.gradient_norm[b] = prog.gradient_norm;
-    }
-    __syncwarp();
+    store_result<T, D>(out, b, lane, x, g, f, prog, nfev);
   }
   if constexpr (kHelpers > 0) {
     if (solver_warp) fn.release_helper(EvalCtx{lane, 0, stage_ptr, slot});

@@ -22,7 +22,7 @@
 
 #include "cno_device.cuh"
 #include "cno_kernel_params.h"
-#include "cno_lbfgs.cuh"
+#include "cno_progress.cuh"
 #include "cno_linesearch.cuh"
 
 namespace cno {
@@ -312,13 +312,7 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
     T gamma = T(1);
     T xx;
     ProgressState<T> prog;
-    prog.x_delta = prog.f_delta = prog.gradient_norm = T(0);
-    prog.num_iterations = 0;
-    prog.x_delta_violations = 0;
-    prog.f_delta_violations = 0;
-    prog.ring_size = 0;
-    prog.ring_pos = 0;
-    prog.status = CNO_STATUS_NOT_STARTED;
+    progress_start(prog);
     // ---- solver.h:189-192: evaluate once at the start point; ||x||^2 of lbfgs.h:95 in the same round ----
     load_quad<T, true>(x0 + b * D + e0, x);
     warp_sum2_p<P, T, E>(fn.partial(ctx, x, &g), lane_dot_p<P, T, E>(x, x), rc, f, xx);
@@ -464,18 +458,9 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
       progress_update<T>(prog, stop, ring, lane, prev_value, f, x_delta, gnorm_inf, x_inf);
     } while (uni(prog.status == CNO_STATUS_CONTINUE));
 
-    // ---- write the returned FunctionState + Progress ----
     if (out.x) store_quad<T>(out.x + b * D + e0, x);
     if (out.gradient) store_quad<T>(out.gradient + b * D + e0, g);
-    if (t == 0) {
-      if (out.value) out.value[b] = f;
-      if (out.num_iterations) out.num_iterations[b] = prog.num_iterations;
-      if (out.status) out.status[b] = (int8_t)prog.status;
-      if (out.nfev) out.nfev[b] = nfev;
-      if (out.x_delta) out.x_delta[b] = prog.x_delta;
-      if (out.f_delta) out.f_delta[b] = prog.f_delta;
-      if (out.gradient_norm) out.gradient_norm[b] = prog.gradient_norm;
-    }
+    if (t == 0) store_result_scalars<T>(out, b, f, prog, nfev);
     __syncwarp();
   }
 }

@@ -32,7 +32,7 @@
 
 #include "cno_device.cuh"
 #include "cno_kernel_params.h"
-#include "cno_lbfgs.cuh"  // ProgressState / progress_update
+#include "cno_progress.cuh"
 #include "cno_linesearch.cuh"
 
 namespace cno {
@@ -182,9 +182,7 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
   };
 
   for (;;) {
-    unsigned long long b = 0;
-    if (lane == 0) b = atomicAdd(queue, 1ULL);
-    b = __shfl_sync(kFullMask, b, 0);
+    const unsigned long long b = claim_instance(queue, lane);
     if (uni(b >= (unsigned long long)batch)) break;
     const EvalCtx ctx{lane, (long long)b, nullptr};
 
@@ -220,13 +218,7 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
     auto slot = [&](int i) -> int { const int s2 = base + i; return s2 >= M ? s2 - M : s2; };
 
     ProgressState<T> prog;
-    prog.num_iterations = 0;
-    prog.x_delta_violations = 0;
-    prog.f_delta_violations = 0;
-    prog.x_delta = prog.f_delta = prog.gradient_norm = T(0);
-    prog.ring_size = 0;
-    prog.ring_pos = 0;
-    prog.status = CNO_STATUS_NOT_STARTED;
+    progress_start(prog);
     StopParams<T> stop_nograd = stop;  // :254-256: the base class's full-gradient test is suppressed
     stop_nograd.gradient_norm = T(0);
     const T pg_tol = stop.gradient_norm;
@@ -620,18 +612,7 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
       if ((pg_tol > T(0)) && (last_pg < pg_tol)) prog.status = CNO_STATUS_GRADIENT_NORM_VIOLATION;
     } while (uni(prog.status == CNO_STATUS_CONTINUE));
 
-    if (out.x) store_row<T, D>(out.x + b * D, lane, x);
-    if (out.gradient) store_row<T, D>(out.gradient + b * D, lane, g);
-    if (lane == 0) {
-      if (out.value) out.value[b] = f;
-      if (out.num_iterations) out.num_iterations[b] = prog.num_iterations;
-      if (out.status) out.status[b] = (int8_t)prog.status;
-      if (out.nfev) out.nfev[b] = nfev;
-      if (out.x_delta) out.x_delta[b] = prog.x_delta;
-      if (out.f_delta) out.f_delta[b] = prog.f_delta;
-      if (out.gradient_norm) out.gradient_norm[b] = prog.gradient_norm;
-    }
-    __syncwarp();
+    store_result<T, D>(out, b, lane, x, g, f, prog, nfev);
   }
 }
 

@@ -32,8 +32,9 @@
 #define CNO_NEWTON_CUH_
 
 #include "cno_device.cuh"
+#include "cno_functors.cuh"  // RosenbrockFn: the value and gradient of RosenbrockFullFn
 #include "cno_kernel_params.h"
-#include "cno_lbfgs.cuh"  // ProgressState / progress_update
+#include "cno_progress.cuh"
 
 namespace cno {
 
@@ -736,14 +737,11 @@ newton_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   __syncwarp();
 
   // (the work queue is read one instance ahead, for the functors that prefetch their next block into L2)
-  unsigned long long bnext = 0;
-  if (lane == 0) bnext = atomicAdd(queue, 1ULL);
-  bnext = __shfl_sync(kFullMask, bnext, 0);
+  unsigned long long bnext = claim_instance(queue, lane);
   for (;;) {
     const unsigned long long b = bnext;
     if (uni(b >= (unsigned long long)batch)) break;
-    if (lane == 0) bnext = atomicAdd(queue, 1ULL);
-    bnext = __shfl_sync(kFullMask, bnext, 0);
+    bnext = claim_instance(queue, lane);
     const EvalCtx ctx{lane, (long long)b, nullptr};
 
     T x[E], g[E];
@@ -760,13 +758,7 @@ newton_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     for (int e = 0; e < E; ++e) vpos[e] = lane * E + e;
 
     ProgressState<T> prog;
-    prog.num_iterations = 0;
-    prog.x_delta_violations = 0;
-    prog.f_delta_violations = 0;
-    prog.x_delta = prog.f_delta = prog.gradient_norm = T(0);
-    prog.ring_size = 0;
-    prog.ring_pos = 0;
-    prog.status = CNO_STATUS_NOT_STARTED;
+    progress_start(prog);
     bool staged = true;  // the store currently holds the unshifted H(x)
 
     do {  // solver.h:196-220
@@ -853,18 +845,7 @@ newton_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       }
     } while (uni(prog.status == CNO_STATUS_CONTINUE));
 
-    if (out.x) store_row<T, D>(out.x + b * D, lane, x);
-    if (out.gradient) store_row<T, D>(out.gradient + b * D, lane, g);
-    if (lane == 0) {
-      if (out.value) out.value[b] = f;
-      if (out.num_iterations) out.num_iterations[b] = prog.num_iterations;
-      if (out.status) out.status[b] = (int8_t)prog.status;
-      if (out.nfev) out.nfev[b] = nfev;
-      if (out.x_delta) out.x_delta[b] = prog.x_delta;
-      if (out.f_delta) out.f_delta[b] = prog.f_delta;
-      if (out.gradient_norm) out.gradient_norm[b] = prog.gradient_norm;
-    }
-    __syncwarp();
+    store_result<T, D>(out, b, lane, x, g, f, prog, nfev);
   }
 }
 
@@ -933,9 +914,7 @@ condition_hessian_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ xs
   __syncwarp();
 
   for (;;) {
-    unsigned long long b = 0;
-    if (lane == 0) b = atomicAdd(queue, 1ULL);
-    b = __shfl_sync(kFullMask, b, 0);
+    const unsigned long long b = claim_instance(queue, lane);
     if (uni(b >= (unsigned long long)batch)) break;
     const EvalCtx ctx{lane, (long long)b, nullptr};
     T x[E];

@@ -489,14 +489,11 @@ __device__ __forceinline__ void newton_dmma_warp(const Fn& fn, const Mat& M, dou
 
   // The work queue is read ONE INSTANCE AHEAD: while instance b is being solved, the block of the instance this warp
   // takes next is already on its way into L2.
-  unsigned long long bnext = 0;
-  if (lane == 0) bnext = atomicAdd(queue, 1ULL);
-  bnext = __shfl_sync(kFullMask, bnext, 0);
+  unsigned long long bnext = claim_instance(queue, lane);
   for (;;) {
     const unsigned long long b = bnext;
     if (uni(b >= (unsigned long long)batch)) break;
-    if (lane == 0) bnext = atomicAdd(queue, 1ULL);
-    bnext = __shfl_sync(kFullMask, bnext, 0);
+    bnext = claim_instance(queue, lane);
     // (the prefetch itself is issued after the first iteration, see below: with two 33 KB blocks per warp in flight for
     // the whole solve, 6 warps x 132 SMs come to about 52 MB -- the size of the 50 MB L2 -- and the second and third
     // pass over A would miss)
@@ -526,13 +523,7 @@ __device__ __forceinline__ void newton_dmma_warp(const Fn& fn, const Mat& M, dou
     int src[E] = {2 * lane, 2 * lane + 1};
 
     ProgressState<T> prog;
-    prog.num_iterations = 0;
-    prog.x_delta_violations = 0;
-    prog.f_delta_violations = 0;
-    prog.x_delta = prog.f_delta = prog.gradient_norm = T(0);
-    prog.ring_size = 0;
-    prog.ring_pos = 0;
-    prog.status = CNO_STATUS_NOT_STARTED;
+    progress_start(prog);
 
     do {  // solver.h:196-220
       // ---- newton_descent.h:73-76: (H + 1e-5 I) delta = -g; the constant Hessian is factored once per instance ----
@@ -595,18 +586,7 @@ __device__ __forceinline__ void newton_dmma_warp(const Fn& fn, const Mat& M, dou
         prefetch_block_l2(fn.data + bnext * fn.stride, lane);  // the next instance's block, one iteration ahead
     } while (uni(prog.status == CNO_STATUS_CONTINUE));
 
-    if (out.x) store_row<T, D>(out.x + b * D, lane, x);
-    if (out.gradient) store_row<T, D>(out.gradient + b * D, lane, g);
-    if (lane == 0) {
-      if (out.value) out.value[b] = f;
-      if (out.num_iterations) out.num_iterations[b] = prog.num_iterations;
-      if (out.status) out.status[b] = (int8_t)prog.status;
-      if (out.nfev) out.nfev[b] = nfev;
-      if (out.x_delta) out.x_delta[b] = prog.x_delta;
-      if (out.f_delta) out.f_delta[b] = prog.f_delta;
-      if (out.gradient_norm) out.gradient_norm[b] = prog.gradient_norm;
-    }
-    __syncwarp();
+    store_result<T, D>(out, b, lane, x, g, f, prog, nfev);
   }
 }
 

@@ -260,7 +260,7 @@ def test_emulation_reproduces_gpu_validated_kernels(emu, solver, hz, dtype, d, l
     (ob.LBFGS, 0, np.float64, 8), (ob.LBFGS, 1, np.float64, 8), (ob.LBFGS, 0, np.float32, 37), (ob.BFGS, 0, np.float64, 8),
     (ob.GRADIENT_DESCENT, 0, np.float64, 8), (ob.CONJUGATED_GRADIENT_DESCENT, 0, np.float64, 8)])
 def test_emulated_kernels_follow_progress_update_under_random_settings(emu, solver, hz, dtype, d):
-    """The device progress_update (csrc/cno_lbfgs.cuh: the order of Progress::Update's tests, the allowed-violation
+    """The device progress_update (csrc/cno_progress.cuh: the order of Progress::Update's tests, the allowed-violation
     counters, relative thresholds, the past-f ring and its square-root-free plateau pre-test) against the oracle under
     six random Progress settings per kernel family -- every output bit for bit."""
     rng = np.random.default_rng(77 + 10 * solver + hz + d)
