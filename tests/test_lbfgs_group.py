@@ -78,17 +78,21 @@ def test_oracle_reproduces_fixture(d):
 
 # ---------------------------------------------------------------- emulation (CPU) ----
 
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """tests/emu/emu_lbfgs_group.cc compiled with the flags of tests/emu/Makefile into a temporary directory."""
-    out = tmp_path_factory.mktemp("emu_group") / "libcno_emu_group.so"
+def build_emu_group(out_dir):
+    """tests/emu/emu_lbfgs_group.cc compiled with the flags of tests/emu/Makefile into `out_dir`."""
+    out = os.path.join(str(out_dir), "libcno_emu_group.so")
     subprocess.run(["g++", "-std=c++20", "-O1", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-pthread",
                     "-DCNO_WARP_EMULATION", "-Wno-unknown-pragmas", "-Wno-attributes", "-shared", "-I", EMU_DIR,
                     "-I", CSRC, "-I", os.path.join(HERE, "..", "include"), "-x", "c++",
-                    os.path.join(EMU_DIR, "emu_lbfgs_group.cc"), "-o", str(out)], check=True)
-    lib = C.CDLL(str(out))
+                    os.path.join(EMU_DIR, "emu_lbfgs_group.cc"), "-o", out], check=True)
+    lib = C.CDLL(out)
     lib.emu_group_sum.argtypes = [C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]
     return lib
+
+
+@pytest.fixture(scope="module")
+def emu(tmp_path_factory):
+    return build_emu_group(tmp_path_factory.mktemp("emu_group"))
 
 
 def _emulated(emu, x0, stop):

@@ -100,31 +100,26 @@ def test_gpu_reproduces_fixture(d):
     bitwise_equal(g, {k: z[k] for k in KEYS})
 
 
-def rare_starts(d):
-    """NaN start, x = 1 (g = 0), a spiked start that takes the +g fallback, and a start 1e-12 off the minimiser
-    (skipped and refused pairs)."""
-    nan = ob.fill_uniform((1, d), 0, 4, -2.0, 2.0)
-    nan[0, d // 3] = np.nan
-    spike = ob.fill_uniform((1, d), 0, 21, -2.0, 2.0)
-    spike[:, ::16] *= 1e12
-    near = 1.0 + 1e-12 * ob.fill_uniform((1, d), 0, 24, -1.0, 1.0)
-    return np.concatenate([nan, np.ones((1, d)), spike, near])
-
-
 @pytest.mark.parametrize("d", DS)
 def test_groups_are_isolated(d):
-    """Rare starts mixed into a batch of 3 * SMs * groups + 5 ordinary rows equal the same starts solved alone."""
-    rare = rare_starts(d)
-    B = 3 * sms() * GROUPS[d] + 5
-    x0 = ob.fill_uniform((B, d), 0, 300 + d, -2.0, 2.0)
-    rows = np.arange(2, B, 11)
-    x0[rows] = rare[np.arange(len(rows)) % len(rare)]
-    g, _ = minimize_c(x0)
-    for r in rows[:2 * len(rare)]:
-        alone, _ = minimize_c(x0[r:r + 1])
-        bitwise_equal({k: v[r:r + 1] for k, v in g.items()}, alone)
-    bitwise_equal({k: v[rows[:len(rare)]] for k, v in g.items()},
-                  ob.minimize(ob.LBFGS, ob.FN_ROSENBROCK, x0[rows[:len(rare)]]))
+    """Each rare-path case of test_lbfgs_group_rare_paths (skipped and refused pairs; usable and skipped pairs in one
+    history; the fallback with one pair and with none; a non-finite trial; a NaN coordinate; x = 1), which first
+    proves from the oracle's path counts that it reaches its branches, mixed into a batch of 3 * SMs * groups + 5
+    ordinary rows under the case's own stop: the rare rows equal the same starts solved alone, and the oracle."""
+    from test_lbfgs_group_rare_paths import KINDS, assert_case_reached, case
+    for kind in KINDS:
+        rare, stop, _ = case(d, kind)
+        B = 3 * sms() * GROUPS[d] + 5
+        x0 = ob.fill_uniform((B, d), 0, 300 + d, -2.0, 2.0)
+        rows = np.arange(2, B, 11)
+        x0[rows] = rare[np.arange(len(rows)) % len(rare)]
+        g, _ = minimize_c(x0, stop)
+        for r in rows[:2 * len(rare)]:
+            alone, _ = minimize_c(x0[r:r + 1], stop)
+            bitwise_equal({k: v[r:r + 1] for k, v in g.items()}, alone)
+        o, paths = ob.lbfgs_paths(ob.FN_ROSENBROCK, x0[rows[:len(rare)]], stop=stop)
+        assert_case_reached(kind, o, paths)
+        bitwise_equal({k: v[rows[:len(rare)]] for k, v in g.items()}, o)
 
 
 @pytest.mark.parametrize("d", DS)
@@ -221,19 +216,41 @@ int main() {
     assert [float(v) for _, _, v in got] == o["value"].tolist()
 
 
-@pytest.fixture(scope="module")
-def one_warp(tmp_path_factory):
-    """tests/cpp/one_warp_rosenbrock.cu: the one-warp kernel on the same objective as a user functor."""
-    out = tmp_path_factory.mktemp("one_warp") / "libcno_one_warp.so"
+def build_one_warp(out_dir):
+    """tests/cpp/one_warp_rosenbrock.cu compiled into `out_dir`: the one-warp kernel on the same objective as a user
+    functor."""
+    out = os.path.join(str(out_dir), "libcno_one_warp.so")
     cuda = os.environ.get("CUDA_HOME", "/usr/local/cuda")
     lib = os.path.join(ROOT, "cppnumericalsolvers_b200")
     subprocess.run([os.environ.get("NVCC", f"{cuda}/bin/nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O3",
                     "-std=c++17", "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false", "-shared",
                     "-Xcompiler", "-fPIC", os.path.join(HERE, "cpp", "one_warp_rosenbrock.cu"),
-                    "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(lib, "csrc"), "-o", str(out),
+                    "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(lib, "csrc"), "-o", out,
                     f"-L{lib}", "-lcno", "-Xlinker", f"-rpath={lib}"], check=True)
     _lib.lib()
-    return C.CDLL(str(out))
+    return C.CDLL(out)
+
+
+@pytest.fixture(scope="module")
+def one_warp(tmp_path_factory):
+    return build_one_warp(tmp_path_factory.mktemp("one_warp"))
+
+
+def minimize_one_warp(one_warp, x0, stop=None):
+    """cno_one_warp_rosenbrock_minimize on x0 -> host outputs."""
+    B, d = x0.shape
+    xd = torch.from_numpy(np.ascontiguousarray(x0)).to(DEV)
+    t = _outputs(B, d)
+    out = _lib.BatchOut(*[t[k].data_ptr() for k in ("x", "value", "gradient", "num_iterations", "status", "nfev",
+                                                     "x_delta", "f_delta", "gradient_norm")])
+    ws = torch.zeros(256, dtype=torch.uint8, device=DEV)
+    stop = stop if stop is not None else ob.default_stop()
+    rc = one_warp.cno_one_warp_rosenbrock_minimize(d, C.c_int64(B), C.c_void_p(xd.data_ptr()), C.byref(stop),
+                                                   C.byref(out), C.c_void_p(ws.data_ptr()), C.c_size_t(256),
+                                                   C.c_void_p(torch.cuda.current_stream().cuda_stream), None)
+    assert rc == 0
+    torch.cuda.synchronize()
+    return _host(t)
 
 
 @pytest.mark.parametrize("d", DS)
@@ -241,15 +258,4 @@ def test_one_warp_user_functor_is_bit_identical(one_warp, d):
     B = 2 * sms() + 3
     x0 = ob.fill_uniform((B, d), 0, 11, -2.0, 2.0)
     group, _ = minimize_c(x0)
-    xd = torch.from_numpy(x0).to(DEV)
-    t = _outputs(B, d)
-    out = _lib.BatchOut(*[t[k].data_ptr() for k in ("x", "value", "gradient", "num_iterations", "status", "nfev",
-                                                     "x_delta", "f_delta", "gradient_norm")])
-    ws = torch.zeros(256, dtype=torch.uint8, device=DEV)
-    stop = ob.default_stop()
-    rc = one_warp.cno_one_warp_rosenbrock_minimize(d, C.c_int64(B), C.c_void_p(xd.data_ptr()), C.byref(stop),
-                                                   C.byref(out), C.c_void_p(ws.data_ptr()), C.c_size_t(256),
-                                                   C.c_void_p(torch.cuda.current_stream().cuda_stream), None)
-    assert rc == 0
-    torch.cuda.synchronize()
-    bitwise_equal(_host(t), group)
+    bitwise_equal(minimize_one_warp(one_warp, x0), group)

@@ -67,7 +67,8 @@ SPIKES = {37: [(11.5, 4, 0), (12.0, 1, 6), (17.5, 37, 2)], 128: [(11.5, 16, 5), 
 
 # (kernel, kind) -> (x0, stop, claims).  Claims: "skip_warmup" / "skip_full" = skipped pairs at k < m / k = m in each
 # position from the newest pair (0, 1, >= 2); "rejected" = refused pairs with a non-empty history; "fallback_reg" =
-# a fallback while every pair of the history was in registers (1 <= k <= R).
+# a fallback while every pair of the history was in registers (1 <= k <= R; k = 1 when R = 0); "fallback_0" /
+# "nonfinite_0" = a fallback / a non-finite trial value with an empty history (k = 0).
 NEAR = ("skip_warmup", "skip_full", "rejected")
 NEAR_ROWS = {"d128_m10": ([1], 150), "d37_m20": ([0], 120), "d128_m20": ([1], 120), "d128_m10_eigen": ([1], 150)}
 
@@ -103,6 +104,10 @@ def assert_reached(paths, regs, claims):
         elif c == "fallback_reg":
             fb = paths["fallback"].sum(0)
             assert fb[1:max(regs, 1) + 1].sum() > 0, ("fallbacks by mem_count", fb)
+        elif c == "fallback_0":
+            assert paths["fallback"].sum(0)[0] > 0, ("fallbacks by mem_count", paths["fallback"].sum(0))
+        elif c == "nonfinite_0":
+            assert paths["nonfinite"].sum(0)[0] > 0, ("non-finite trials by mem_count", paths["nonfinite"].sum(0))
         else:
             raise AssertionError(c)
 
