@@ -65,18 +65,137 @@ struct LbfgsSmem {
   static constexpr size_t kBytes = kWarpBytes * kWarps;
 };
 
-// y-history accessor: the warp's shared-memory slice (chunk-interleaved).  A load is issued before the reduction it
-// overlaps and consumed after it (issue / wait).
-template <class T, int E>
-struct YHist {
-  T* base;
-  int lane;
-  struct Pending {};
-  __device__ __forceinline__ void store(int slot, const T (&v)[E]) const { SmemVec<T, E>::store(base + slot * 32 * E, lane, v); }
-  __device__ __forceinline__ void issue(int slot, T (&v)[E], Pending&) const { SmemVec<T, E>::load(base + slot * 32 * E, lane, v); }
-  __device__ __forceinline__ void wait(T (&)[E], Pending&) const {}
-  __device__ __forceinline__ void fence_store() const {}
+// ---- the steps of Lbfgs::OptimizationStep shared by lbfgs_minimize_kernel and the group kernel
+//      (cno_lbfgs_group.cuh); RC is the reduction context, RedCtx<T> or GroupCtx<T, W> ----
+
+// Which (s, y) pairs the history holds: mem_count pairs, chronological i = 0 (oldest) .. mem_count - 1.  Pair i lives in
+// register slot mem_count - 1 - i if that is below R (the newest), else in slot (mem_pos + i) mod MS of the shared ring;
+// mem_pos stays 0 until the ring is full.  At R = 0 this is the reference's index map (lbfgs.h:162).
+template <int M, int R = 0>
+struct LbfgsHistory {
+  static constexpr int MS = M - R;  // slots of the shared ring
+  int mem_count, mem_pos;
+  unsigned valid;  // bit i set <=> !(|s_i . y_i| < eps), i chronological  (lbfgs.h:165,189)
+  __device__ __forceinline__ void clear() {
+    mem_count = 0;
+    mem_pos = 0;
+    valid = 0;
+  }
+  __device__ __forceinline__ bool pair_usable(int i) const { return (valid >> i) & 1u; }
+  // The ring slot of the pair that enters the shared ring (mem_count >= R): the oldest register pair, or (R = 0) the
+  // new one; when the ring is full it replaces the oldest pair there, which leaves the history.
+  __device__ __forceinline__ int ring_slot() {
+    int slot = mem_count - R;
+    if (slot == MS) {
+      slot = mem_pos;
+      mem_pos = (mem_pos + 1 == MS) ? 0 : mem_pos + 1;
+    }
+    return slot;
+  }
+  // a new pair with s.y = sy joins the history (lbfgs.h:269-279) with its bit of `valid`
+  template <class T>
+  __device__ __forceinline__ void record(T sy) {
+    const unsigned usable = (cabs(sy) < Num<T>::eps) ? 0u : 1u;
+    if (mem_count < M) {
+      valid |= usable << mem_count;
+      mem_count++;
+    } else {
+      valid = (valid >> 1) | (usable << (M - 1));
+    }
+  }
 };
+
+// Descent test, alpha_init and fallback (lbfgs.h:199-224) on the two-loop direction q.  Returns dginit = g.(-q): the
+// search runs along -q (the line search negates inside its products, cno_linesearch.cuh kNeg), so no negated copy of q
+// is ever made.  The fallback sets q = -g and empties the history (register pairs included).
+template <class P, class T, int E, int M, int R, class RC>
+__device__ __forceinline__ T lbfgs_direction(const RC& rc, const T (&g)[E], T (&q)[E], const T xx,
+                                             LbfgsHistory<M, R>& h, T& alpha_init) {
+  constexpr T eps = Num<T>::eps;
+  alpha_init = T(1);
+  T gq;
+  if (uni(h.mem_count == 0)) {  // :208-213 (||q|| only matters without history)
+    T qq;
+    warp_sum2_p<P, T, E>(lane_dot_p<P, T, E>(g, q), lane_dot_p<P, T, E>(q, q), rc, gq, qq);
+    const T qn = csqrt(qq);
+    alpha_init = (qn > eps) ? T(1) / qn : T(1);
+  } else {
+    gq = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(g, q), rc);
+  }
+  const T descent_direction = -gq;
+  T dginit = descent_direction;  // = g.(-q), bit for bit
+  // descent_direction > -eps * relative_eps, relative_eps = eps * max(1, ||x||) (:93-95)?  |eps * relative_eps| <=
+  // eps^2 max(1, ||x||) (1 + 2^-50) and sqrt(t) <= max(1, t), so a finite direction below -2 eps^2 max(1, x.x) is below
+  // the exact threshold whatever its rounding: the comparison is false and neither the square root nor the products
+  // are needed.  Anything else (a non-finite operand, a direction that close to zero) takes the specification's
+  // expression.
+  bool fallback;
+  if (cfinite(descent_direction) && cfinite(xx) && descent_direction < -(T(2) * eps * eps) * smax(T(1), xx)) {
+    fallback = false;
+  } else {
+    const T relative_eps = eps * smax(T(1.0), csqrt(xx));
+    fallback = !cfinite(descent_direction) || descent_direction > -eps * relative_eps;
+  }
+  if (uni(fallback)) {
+    // search_direction = -g, and the reference then searches along -search_direction = +g (SURVEY.md 7.2a):
+    // dginit = g.g >= 0.
+#pragma unroll
+    for (int j = 0; j < E; ++j) q[j] = -g[j];
+    h.clear();
+    const T gg = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(g, g), rc);  // :221 (rare path)
+    const T gn = csqrt(gg);
+    alpha_init = (gn > eps) ? T(1) / gn : T(1);
+    dginit = gg;
+  }
+  return dginit;
+}
+
+// MoreThuente::Search / HagerZhang (lbfgs.h:231-232) along -q, its evaluations added to nfev, or the search's own
+// early return for dginit >= 0 (more_thuente.h:152-156): the state untouched.
+template <class LS, class Fn, class T, int E, class RC>
+__device__ __forceinline__ void lbfgs_search(const Fn& fn, const EvalCtx& ctx, const RC& rc, const T (&x)[E],
+                                             const T f, const T (&g)[E], T (&xn)[E], T& fn_val, T (&gn)[E],
+                                             const T alpha_init, const T (&q)[E], const T dginit, uint32_t& nfev) {
+  if (uni(dginit >= T(0))) {
+#pragma unroll
+    for (int j = 0; j < E; ++j) { xn[j] = x[j]; gn[j] = g[j]; }
+    fn_val = f;
+  } else {
+    nfev += LS::template search<Fn, T, E, true, std::is_same<LS, LsMoreThuente>::value>(fn, ctx, rc, x, f, g, xn,
+                                                                                        fn_val, gn, alpha_init, q,
+                                                                                        dginit);
+  }
+}
+
+// s.y, s.s, y.y (:265-266) and the next step's ||x||^2 (:95), reduced together.  Returns s.y > eps ||s|| ||y|| (:266),
+// decided without the two square roots whenever a rigorous bound allows.
+template <class P, class T, int E, class RC>
+__device__ __forceinline__ bool lbfgs_pair_sums(const RC& rc, const T (&sd)[E], const T (&yd)[E], const T (&xn)[E],
+                                                T& sy, T& yy, T& xx_next) {
+  T ss;
+  warp_sum4_p<P, T, E>(lane_dot_p<P, T, E>(sd, yd), lane_dot_p<P, T, E>(sd, sd), lane_dot_p<P, T, E>(yd, yd),
+                       lane_dot_p<P, T, E>(xn, xn), rc, sy, ss, yy, xx_next);
+  return curvature_above_eps<T>(sy, ss, yy);
+}
+
+// gamma = s.y / y.y when that is usable (lbfgs.h:289-298)
+template <class T>
+__device__ __forceinline__ void lbfgs_update_gamma(T& gamma, const T sy, const T yy) {
+  constexpr T eps = Num<T>::eps;
+  if (yy > eps) {
+    const T temp_scaling = sy / yy;
+    if (cfinite(temp_scaling) && cabs(temp_scaling) <= T(1e7)) gamma = smax(temp_scaling, eps);
+  }
+}
+
+// lpNorm<Infinity> of three vectors of one warp (the GroupCtx overload is in cno_lbfgs_group.cuh).
+template <class T, int E>
+__device__ __forceinline__ void maxabs3(const RedCtx<T>&, const T (&a)[E], const T (&b)[E], const T (&c)[E], T& ra,
+                                        T& rb, T& rc_out) {
+  ra = warp_maxabs<T, E>(a);
+  rb = warp_maxabs<T, E>(b);
+  rc_out = warp_maxabs<T, E>(c);
+}
 
 // Record of one parked instance (stepwise solves): S slots, Y slots (lane-major),
 // then scalars.  What Lbfgs keeps as members between OptimizationStep calls
@@ -163,9 +282,8 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
   // the instance slot this warp works for: its own, or (helper warps) the one of its solver warp
   const int slot = (kHelpers > 0 && warp >= SM::kHelperBase) ? warp - SM::kHelperBase : warp;
   T* const S = reinterpret_cast<T*>(smem_raw) + (size_t)slot * SM::kWarpElems;
+  T* const Y = S + MS * SM::kVec;
   T* const rho_s = S + 2 * MS * SM::kVec;  // 1 / (s_i . y_i) per slot
-  const YHist<T, E> Y{S + MS * SM::kVec, lane};
-  typename YHist<T, E>::Pending ypend;
   T* const alpha = rho_s + MS;
   T* const ring = alpha + MS;
   // policy scratch (PolicyEigenSSE2): 16-byte aligned tail of the scalar block; handed to
@@ -196,12 +314,8 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     T x[E], g[E];
     T f;
     uint32_t nfev;
-    // mem_count pairs, chronological i = 0 (oldest) .. mem_count - 1.  Pair i lives in register slot
-    // mem_count - 1 - i if that is below R (rs/ry/rrho[0]: the newest), else in shared slot (mem_pos + i) mod MS;
-    // mem_pos stays 0 until the ring is full.  At R = 0 this is the reference's index map (lbfgs.h:162).
-    int mem_count, mem_pos;
-    unsigned valid;  // bit i set <=> !(|s_i . y_i| < eps), i chronological  (lbfgs.h:165,189)
-    T rs[RA][E], ry[RA][E], rrho[RA];
+    LbfgsHistory<M, R> hist;
+    T rs[RA][E], ry[RA][E], rrho[RA];  // the register pairs, [0] the newest
     T gamma;
     T xx;            // ||x||^2 carried across iterations (the dot the reference recomputes at lbfgs.h:95)
     ProgressState<T> prog;
@@ -223,9 +337,9 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         if (lane < CNO_MAX_PAST) ring[lane] = sc[M + lane];
         gamma = sc[M + CNO_MAX_PAST];
         xx = sc[M + CNO_MAX_PAST + 1];
-        mem_count = in[0];
-        mem_pos = in[1];
-        valid = (unsigned)in[2];
+        hist.mem_count = in[0];
+        hist.mem_pos = in[1];
+        hist.valid = (unsigned)in[2];
         prog.num_iterations = (uint32_t)in[3];
         prog.x_delta_violations = in[4];
         prog.f_delta_violations = in[5];
@@ -239,9 +353,8 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           load_row<T, 32 * E, false>(reinterpret_cast<const T*>(rec + RL::kS) + slot * 32 * E, lane, v);
           SV::store(S + slot * SM::kVec, lane, v);
           load_row<T, 32 * E, false>(reinterpret_cast<const T*>(rec + RL::kY) + slot * 32 * E, lane, v);
-          Y.store(slot, v);
+          SV::store(Y + slot * SM::kVec, lane, v);
         }
-        Y.fence_store();
         __syncwarp();
         resumed = true;
       }
@@ -252,9 +365,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       f = fn(ctx, x, &g);
       nfev = 1;
       // ---- lbfgs.h:72-87 InitializeSolver ----
-      mem_count = 0;
-      mem_pos = 0;
-      valid = 0;
+      hist.clear();
       gamma = T(1);
       xx = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(x, x), rc);
     }
@@ -262,9 +373,6 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
 
     do {  // solver.h:196-220
       // ================= Lbfgs::OptimizationStep (lbfgs.h:89-303) =========
-      // relative_eps = eps * max(1, ||x||) (:93-95) enters ONE comparison, the descent test below; it is formed there,
-      // and only when a square-root-free bound does not already decide the comparison.
-
       // Second mode (:129-135): M^-1 = 1 / (|diag H| + eps); the gradient the reference
       // re-evaluates there is the state's gradient (same function, same x, same bits).
       T precond[E];
@@ -277,17 +385,17 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       T q[E];  // search_direction
 #pragma unroll
       for (int j = 0; j < E; ++j) q[j] = g[j];  // :145
-      const int k = mem_count;
+      const int k = hist.mem_count;
 
       // ================= two-loop recursion (:157-196) =====================
-      // Pairs in chronological order (see mem_count): loop 1 takes the register pairs, then the shared ones;
+      // Pairs in chronological order (see LbfgsHistory): loop 1 takes the register pairs, then the shared ones;
       // loop 2 the reverse.  In both loops the loads of the next shared pair are issued before the current
       // reduction (the reduction is the critical path; LDS latency hides under it).
       T ra[RA];  // alpha of the register pairs
-      if (uni(k == M && valid == ((1u << M) - 1u))) {
+      if (uni(k == M && hist.valid == ((1u << M) - 1u))) {
         // ---- steady state (full history, every pair usable): both loops fully
         //      unrolled, alpha_i in registers, no per-pair control flow ----
-        int idx = mem_pos + MS - 1;
+        int idx = hist.mem_pos + MS - 1;
         idx = (idx >= MS) ? idx - MS : idx;
         T sv[E], yv[E];
         if (R == 0) SV::load(S + idx * SM::kVec, lane, sv);
@@ -304,11 +412,10 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           const int idx_next = (idx == 0) ? MS - 1 : idx - 1;
           const auto part = lane_dot_p<P, T, E>(sv, q);
           const T r = rho_s[idx];
-          Y.issue(idx, yv, ypend);
+          SV::load(Y + idx * SM::kVec, lane, yv);
           if (i > 0) SV::load(S + idx_next * SM::kVec, lane, sv);
           const T a = r * warp_sum_p<P, T, E>(part, rc);
           if (lane == 0) alpha[i] = a;
-          Y.wait(yv, ypend);
 #pragma unroll
           for (int j = 0; j < E; ++j) q[j] = q[j] - a * yv[j];
           idx = idx_next;
@@ -316,7 +423,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         __syncwarp();
 #pragma unroll
         for (int j = 0; j < E; ++j) q[j] = kSecond ? (precond[j] * q[j]) : (q[j] * gamma);  // H0 (:177-182)
-        idx = mem_pos;
+        idx = hist.mem_pos;
         // (yv still holds y of the oldest pair: the last pair of loop 1 is the first of loop 2)
 #pragma unroll
         for (int i = 0; i < MS; ++i) {  // second loop (:185-196), shared pairs: oldest first
@@ -325,12 +432,11 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           const T r = rho_s[idx];
           const T al = alpha[i];
           SV::load(S + idx * SM::kVec, lane, sv);
-          if (i + 1 < MS) Y.issue(idx_next, yv, ypend);
+          if (i + 1 < MS) SV::load(Y + idx_next * SM::kVec, lane, yv);
           const T beta = r * warp_sum_p<P, T, E>(part, rc);
           const T coef = al - beta;
 #pragma unroll
           for (int j = 0; j < E; ++j) q[j] = q[j] + sv[j] * coef;
-          if (i + 1 < MS) Y.wait(yv, ypend);
           idx = idx_next;
         }
 #pragma unroll
@@ -351,7 +457,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           if (uni(j < kr)) {
             const auto part = lane_dot_p<P, T, E>(rs[j], q);
             const T a = rrho[j] * warp_sum_p<P, T, E>(part, rc);
-            if (uni((valid >> (k - 1 - j)) & 1u)) {  // lbfgs.h:165 skip
+            if (uni(hist.pair_usable(k - 1 - j))) {  // lbfgs.h:165 skip
               ra[j] = a;
 #pragma unroll
               for (int e = 0; e < E; ++e) q[e] = q[e] - a * ry[j][e];
@@ -359,7 +465,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           }
         }
         if (uni(ks > 0)) {
-          int idx = mem_pos + ks - 1;
+          int idx = hist.mem_pos + ks - 1;
           idx = (idx >= MS) ? idx - MS : idx;
           T sv[E];
           SV::load(S + idx * SM::kVec, lane, sv);
@@ -368,11 +474,10 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
             const int idx_next = (idx == 0) ? MS - 1 : idx - 1;
             const auto part = lane_dot_p<P, T, E>(sv, q);
             T yv[E];
-            Y.issue(idx, yv, ypend);
+            SV::load(Y + idx * SM::kVec, lane, yv);
             SV::load(S + idx_next * SM::kVec, lane, sv);  // prefetch (harmless at i == 0)
             const T a = rho_s[idx] * warp_sum_p<P, T, E>(part, rc);
-            Y.wait(yv, ypend);
-            if (uni((valid >> i) & 1u)) {  // lbfgs.h:165 skip
+            if (uni(hist.pair_usable(i))) {  // lbfgs.h:165 skip
               if (lane == 0) alpha[i] = a;
   #pragma unroll
               for (int j = 0; j < E; ++j) q[j] = q[j] - a * yv[j];
@@ -386,20 +491,18 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         for (int j = 0; j < E; ++j) q[j] = kSecond ? (precond[j] * q[j]) : (q[j] * gamma);
         // ---- second loop (:185-196): oldest pair first ----
         if (uni(ks > 0)) {
-          int idx = mem_pos;
+          int idx = hist.mem_pos;
           T yv[E];
-          Y.issue(idx, yv, ypend);
-          Y.wait(yv, ypend);
+          SV::load(Y + idx * SM::kVec, lane, yv);
   #pragma unroll 1
           for (int i = 0; uni(i < ks); ++i) {
             const int idx_next = (idx + 1 == MS) ? 0 : idx + 1;
             const auto part = lane_dot_p<P, T, E>(yv, q);
             T sv[E];
             SV::load(S + idx * SM::kVec, lane, sv);
-            Y.issue(idx_next, yv, ypend);  // prefetch (harmless past the end: a valid slot)
+            SV::load(Y + idx_next * SM::kVec, lane, yv);  // prefetch (harmless past the end: a valid slot)
             const T beta = rho_s[idx] * warp_sum_p<P, T, E>(part, rc);
-            Y.wait(yv, ypend);
-            if (uni((valid >> i) & 1u)) {  // lbfgs.h:189 skip
+            if (uni(hist.pair_usable(i))) {  // lbfgs.h:189 skip
               const T coef = alpha[i] - beta;
   #pragma unroll
               for (int j = 0; j < E; ++j) q[j] = q[j] + sv[j] * coef;
@@ -412,7 +515,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           if (uni(j < kr)) {
             const auto part = lane_dot_p<P, T, E>(ry[j], q);
             const T beta = rrho[j] * warp_sum_p<P, T, E>(part, rc);
-            if (uni((valid >> (k - 1 - j)) & 1u)) {  // lbfgs.h:189 skip
+            if (uni(hist.pair_usable(k - 1 - j))) {  // lbfgs.h:189 skip
               const T coef = ra[j] - beta;
 #pragma unroll
               for (int e = 0; e < E; ++e) q[e] = q[e] + rs[j][e] * coef;
@@ -421,99 +524,39 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         }
       }
 
-      // ---- descent test, alpha_init, fallback (:199-224) ----
-      T alpha_init = T(1);
-      T gq;
-      if (uni(mem_count == 0)) {  // :208-213 (||q|| only matters without history)
-        T qq;
-        warp_sum2_p<P, T, E>(lane_dot_p<P, T, E>(g, q), lane_dot_p<P, T, E>(q, q), rc, gq, qq);
-        const T qn = csqrt(qq);
-        alpha_init = (qn > eps) ? T(1) / qn : T(1);
-      } else {
-        gq = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(g, q), rc);
-      }
-      const T descent_direction = -gq;
-      T dginit = descent_direction;  // = g.(-q), bit for bit
-      // The search runs along -q (the line search negates inside its products, cno_linesearch.cuh
-      // kNeg), so no negated copy of q is ever made.
-      // descent_direction > -eps * relative_eps?  |eps * relative_eps| <= eps^2 max(1, ||x||) (1 + 2^-50) and
-      // sqrt(t) <= max(1, t), so a finite direction below -2 eps^2 max(1, x.x) is below the exact threshold whatever
-      // its rounding: the comparison is false and neither the square root nor the products are needed.  Anything else
-      // (a non-finite operand, a direction that close to zero) takes the specification's expression.
-      bool fallback;
-      if (cfinite(descent_direction) && cfinite(xx) && descent_direction < -(T(2) * eps * eps) * smax(T(1), xx)) {
-        fallback = false;
-      } else {
-        const T relative_eps = eps * smax(T(1.0), csqrt(xx));  // :93-95
-        fallback = !cfinite(descent_direction) || descent_direction > -eps * relative_eps;
-      }
-      if (uni(fallback)) {
-        // fallback: search_direction = -g, and the reference then searches
-        // along -search_direction = +g (SURVEY.md 7.2a): dginit = g.g >= 0.
-#pragma unroll
-        for (int j = 0; j < E; ++j) q[j] = -g[j];
-        mem_count = 0;  // (empties the register pairs as well)
-        mem_pos = 0;
-        valid = 0;
-        const T gg = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(g, g), rc);  // :221 (rare path)
-        const T gn = csqrt(gg);
-        alpha_init = (gn > eps) ? T(1) / gn : T(1);
-        dginit = gg;
-      }
-
-      // ---- MoreThuente::Search (:231-232) ----
+      T alpha_init;
+      const T dginit = lbfgs_direction<P>(rc, g, q, xx, hist, alpha_init);
       T xn[E], gn[E];
       T fn_val;
-      if (uni(dginit >= T(0))) {  // the search's own early return (more_thuente.h:152-156): state untouched
-#pragma unroll
-        for (int j = 0; j < E; ++j) { xn[j] = x[j]; gn[j] = g[j]; }
-        fn_val = f;
-      } else {
-        nfev += LS::template search<Fn, T, E, true, std::is_same<LS, LsMoreThuente>::value>(
-            fn, ctx, rc, x, f, g, xn, fn_val, gn, alpha_init, q, dginit);
-      }
+      lbfgs_search<LS>(fn, ctx, rc, x, f, g, xn, fn_val, gn, alpha_init, q, dginit, nfev);
 
       const T prev_value = f;
       T x_delta, gnorm_inf, x_inf;
       if (uni(!cfinite(fn_val))) {
         // :239-241 return current: x, g, f unchanged; x_delta = |x - x|_inf (progress.h:190) is 0,
         // or NaN when x itself holds a non-finite component (rare path, computed as written).
-        gnorm_inf = warp_maxabs<T, E>(g);
-        x_inf = warp_maxabs<T, E>(x);
         T zd[E];
 #pragma unroll
         for (int j = 0; j < E; ++j) zd[j] = x[j] - x[j];
-        x_delta = warp_maxabs<T, E>(zd);
+        maxabs3(rc, zd, g, x, x_delta, gnorm_inf, x_inf);
       } else {
         // ---- pair + gamma update (:248-298) ----
         T sd[E], yd[E];
 #pragma unroll
         for (int j = 0; j < E; ++j) { sd[j] = xn[j] - x[j]; yd[j] = gn[j] - g[j]; }
-        // s.y, s.s, y.y (:265-266) and the next step's ||x||^2 (:95), reduced together
-        T sy, ss, yy, xx_next;
-        warp_sum4_p<P, T, E>(lane_dot_p<P, T, E>(sd, yd), lane_dot_p<P, T, E>(sd, sd),
-                             lane_dot_p<P, T, E>(yd, yd), lane_dot_p<P, T, E>(xn, xn), rc, sy, ss, yy, xx_next);
-        // s.y > eps ||s|| ||y|| (:266), decided without the two square roots whenever a rigorous bound allows
-        const bool curvature_ok = curvature_above_eps<T>(sy, ss, yy);
-        if (uni(curvature_ok)) {
+        T sy, yy, xx_next;
+        if (uni(lbfgs_pair_sums<P>(rc, sd, yd, xn, sy, yy, xx_next))) {
           // s.y is exactly the dot the reference recomputes per use; cache 1/(s.y)
           const T rho_new = T(1) / sy;
-          if (uni(mem_count >= R)) {
-            // a pair enters the shared ring: the oldest register pair, or (R = 0) the new one; when the ring
-            // is full it replaces the oldest pair there, which leaves the history
-            int slot = mem_count - R;
-            if (slot == MS) {
-              slot = mem_pos;
-              mem_pos = (mem_pos + 1 == MS) ? 0 : mem_pos + 1;
-            }
+          if (uni(hist.mem_count >= R)) {
+            const int slot = hist.ring_slot();
             if constexpr (R > 0) {
               SV::store(S + slot * SM::kVec, lane, rs[R - 1]);
-              Y.store(slot, ry[R - 1]);
+              SV::store(Y + slot * SM::kVec, lane, ry[R - 1]);
             } else {
               SV::store(S + slot * SM::kVec, lane, sd);
-              Y.store(slot, yd);
+              SV::store(Y + slot * SM::kVec, lane, yd);
             }
-            Y.fence_store();
             __syncwarp();  // all lanes are done reading rho_s in this iteration's loops
             if (lane == 0) rho_s[slot] = (R > 0) ? rrho[RA - 1] : rho_new;
           }
@@ -528,25 +571,14 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
             for (int e = 0; e < E; ++e) { rs[0][e] = sd[e]; ry[0][e] = yd[e]; }
             rrho[0] = rho_new;
           }
-          const unsigned usable = (cabs(sy) < eps) ? 0u : 1u;
-          if (mem_count < M) {
-            valid |= usable << mem_count;
-            mem_count++;
-          } else {
-            valid = (valid >> 1) | (usable << (M - 1));
-          }
+          hist.record(sy);
         }
-        if (yy > eps) {
-          const T temp_scaling = sy / yy;
-          if (cfinite(temp_scaling) && cabs(temp_scaling) <= T(1e7)) gamma = smax(temp_scaling, eps);
-        }
-        // next state + the norms Progress::Update and the next step need
-        x_delta = warp_maxabs<T, E>(sd);
+        lbfgs_update_gamma(gamma, sy, yy);
+        // the norms Progress::Update and the next step need, then the next state
+        maxabs3(rc, sd, gn, xn, x_delta, gnorm_inf, x_inf);
 #pragma unroll
         for (int j = 0; j < E; ++j) { x[j] = xn[j]; g[j] = gn[j]; }
         f = fn_val;
-        gnorm_inf = warp_maxabs<T, E>(g);
-        x_inf = warp_maxabs<T, E>(x);
         xx = xx_next;
         __syncwarp();
       }
@@ -569,9 +601,9 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         if (lane == 0) {
           sc[M + CNO_MAX_PAST] = gamma;
           sc[M + CNO_MAX_PAST + 1] = xx;
-          in[0] = mem_count;
-          in[1] = mem_pos;
-          in[2] = (int)valid;
+          in[0] = hist.mem_count;
+          in[1] = hist.mem_pos;
+          in[2] = (int)hist.valid;
           in[3] = (int)prog.num_iterations;
           in[4] = prog.x_delta_violations;
           in[5] = prog.f_delta_violations;
@@ -584,8 +616,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           T v[E];
           SV::load(S + slot * SM::kVec, lane, v);
           store_row<T, 32 * E>(reinterpret_cast<T*>(rec + RL::kS) + slot * 32 * E, lane, v);
-          Y.issue(slot, v, ypend);
-          Y.wait(v, ypend);
+          SV::load(Y + slot * SM::kVec, lane, v);
           store_row<T, 32 * E>(reinterpret_cast<T*>(rec + RL::kY) + slot * 32 * E, lane, v);
         }
       }

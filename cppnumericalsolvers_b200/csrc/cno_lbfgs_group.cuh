@@ -15,15 +15,16 @@
 // so all warps hold identical bits without a second broadcast; every scalar is replicated in every warp and every
 // branch is uniform across the group.  The oracle (reduce_dmma_tree) is the same function of the same terms.
 //
+// The iteration runs the one-warp kernel's steps (cno_lbfgs.cuh: LbfgsHistory, lbfgs_direction, lbfgs_search,
+// lbfgs_pair_sums, lbfgs_update_gamma, maxabs3) on a GroupCtx, with the whole history in shared memory (R = 0); the two
+// loops of the recursion and the pair store are the group's own.
+//
 // Not covered: user functors (a block-cooperative functor concept is a public-interface change), register-held pairs,
 // the stepwise (parked) form, Second mode, HagerZhang.
 #ifndef CNO_LBFGS_GROUP_CUH_
 #define CNO_LBFGS_GROUP_CUH_
 
-#include "cno_device.cuh"
-#include "cno_kernel_params.h"
-#include "cno_progress.cuh"
-#include "cno_linesearch.cuh"
+#include "cno_lbfgs.cuh"
 
 namespace cno {
 
@@ -38,8 +39,8 @@ __device__ __forceinline__ void group_bar(int id, int threads) {
 #endif
 }
 
-// The reduction context of a group (the counterpart of RedCtx<T>; the line search takes either).  scratch holds two
-// buffers of kMaxSums x W x 32 sub-partials.  Consecutive collectives alternate between them (`phase`): a warp can only
+// The reduction context of a group (the counterpart of RedCtx<T>; the line search and the L-BFGS steps take either).
+// scratch holds two buffers of kMaxSums x W x 32 sub-partials.  Consecutive collectives alternate between them (`phase`): a warp can only
 // write a buffer again after passing the barrier of the collective in between, which every other warp reaches only
 // after it has read that buffer, so one barrier per collective suffices.
 template <class T, int W>
@@ -106,8 +107,8 @@ __device__ __forceinline__ void warp_sum4_p(const typename LanePartial<P, T, E>:
 // pattern of |v_i| read as an unsigned integer; order free): each warp's maximum, then the maximum over the W warps as
 // 64-bit patterns.
 template <class T, int W>
-__device__ __forceinline__ void group_maxabs3(const GroupCtx<T, W>& rc, const T (&a)[4], const T (&b)[4],
-                                              const T (&c)[4], T& ra, T& rb, T& rc_out) {
+__device__ __forceinline__ void maxabs3(const GroupCtx<T, W>& rc, const T (&a)[4], const T (&b)[4], const T (&c)[4],
+                                        T& ra, T& rb, T& rc_out) {
   static_assert(sizeof(T) == 8, "group maxabs: fp64");
   T* const buf = rc.scratch + rc.phase * GroupCtx<T, W>::kBufElems;
   rc.phase ^= 1;
@@ -265,8 +266,7 @@ struct LbfgsGroupPlan {
   static constexpr size_t kBytes = kGroupBytes * kGroups;
 };
 
-// Lbfgs<Fn, M>::Minimize with MoreThuente, First mode: lbfgs_minimize_kernel (cno_lbfgs.cuh) step for step with the
-// whole history in shared memory (its R = 0 form), on a group functor.
+// Lbfgs<Fn, M>::Minimize with MoreThuente, First mode, on a group functor.
 template <class Fn, int M>
 __global__ void __launch_bounds__(LbfgsGroupPlan<typename Fn::Scalar, Fn::Dim, M>::kThreads, 1)
 lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, const long long batch,
@@ -280,7 +280,6 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
   constexpr int E = 4;
   using P = PolicyFast;
   using GV = GroupVec<T, W>;
-  constexpr T eps = Num<T>::eps;
 
   CNO_DYNAMIC_SMEM(smem_raw);
   const int group = (int)threadIdx.x / NT;
@@ -307,8 +306,8 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
     T x[E], g[E];
     T f;
     uint32_t nfev;
-    int mem_count = 0, mem_pos = 0;  // pair i (chronological) in slot (mem_pos + i) mod M (lbfgs.h:162)
-    unsigned valid = 0;              // bit i set <=> !(|s_i . y_i| < eps)  (lbfgs.h:165,189)
+    LbfgsHistory<M> hist;
+    hist.clear();
     T gamma = T(1);
     T xx;
     ProgressState<T> prog;
@@ -323,10 +322,10 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
       T q[E];
 #pragma unroll
       for (int j = 0; j < E; ++j) q[j] = g[j];  // :145
-      const int k = mem_count;
+      const int k = hist.mem_count;
       // ---- first loop (:157-171): newest pair first ----
       if (uni(k > 0)) {
-        int idx = mem_pos + k - 1;
+        int idx = hist.mem_pos + k - 1;
         idx = (idx >= M) ? idx - M : idx;
 #pragma unroll 1
         for (int i = k - 1; uni(i >= 0); --i) {
@@ -334,7 +333,7 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
           GV::load(S + idx * D, t, sv);
           GV::load(Yh + idx * D, t, yv);
           const T a = rho_s[idx] * warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(sv, q), rc);
-          if (uni((valid >> i) & 1u)) {  // lbfgs.h:165 skip
+          if (uni(hist.pair_usable(i))) {  // lbfgs.h:165 skip
             if (lane == 0) alpha[i] = a;
 #pragma unroll
             for (int j = 0; j < E; ++j) q[j] = q[j] - a * yv[j];
@@ -347,14 +346,14 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
       for (int j = 0; j < E; ++j) q[j] = q[j] * gamma;  // H0 (:177-182)
       // ---- second loop (:185-196): oldest pair first ----
       if (uni(k > 0)) {
-        int idx = mem_pos;
+        int idx = hist.mem_pos;
 #pragma unroll 1
         for (int i = 0; uni(i < k); ++i) {
           T sv[E], yv[E];
           GV::load(Yh + idx * D, t, yv);
           GV::load(S + idx * D, t, sv);
           const T beta = rho_s[idx] * warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(yv, q), rc);
-          if (uni((valid >> i) & 1u)) {  // lbfgs.h:189 skip
+          if (uni(hist.pair_usable(i))) {  // lbfgs.h:189 skip
             const T coef = alpha[i] - beta;
 #pragma unroll
             for (int j = 0; j < E; ++j) q[j] = q[j] + sv[j] * coef;
@@ -363,49 +362,11 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
         }
       }
 
-      // ---- descent test, alpha_init, fallback (:199-224) ----
-      T alpha_init = T(1);
-      T gq;
-      if (uni(mem_count == 0)) {  // :208-213
-        T qq;
-        warp_sum2_p<P, T, E>(lane_dot_p<P, T, E>(g, q), lane_dot_p<P, T, E>(q, q), rc, gq, qq);
-        const T qn = csqrt(qq);
-        alpha_init = (qn > eps) ? T(1) / qn : T(1);
-      } else {
-        gq = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(g, q), rc);
-      }
-      const T descent_direction = -gq;
-      T dginit = descent_direction;
-      bool fallback;
-      if (cfinite(descent_direction) && cfinite(xx) && descent_direction < -(T(2) * eps * eps) * smax(T(1), xx)) {
-        fallback = false;
-      } else {
-        const T relative_eps = eps * smax(T(1.0), csqrt(xx));  // :93-95
-        fallback = !cfinite(descent_direction) || descent_direction > -eps * relative_eps;
-      }
-      if (uni(fallback)) {
-        // search_direction = -g; the reference then searches along +g (SURVEY.md 7.2a): dginit = g.g >= 0
-#pragma unroll
-        for (int j = 0; j < E; ++j) q[j] = -g[j];
-        mem_count = 0;
-        mem_pos = 0;
-        valid = 0;
-        const T gg = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(g, g), rc);  // :221
-        const T gn = csqrt(gg);
-        alpha_init = (gn > eps) ? T(1) / gn : T(1);
-        dginit = gg;
-      }
-
-      // ---- MoreThuente::Search (:231-232), along -q ----
+      T alpha_init;
+      const T dginit = lbfgs_direction<P>(rc, g, q, xx, hist, alpha_init);
       T xn[E], gn[E];
       T fn_val;
-      if (uni(dginit >= T(0))) {  // more_thuente.h:152-156: state untouched
-#pragma unroll
-        for (int j = 0; j < E; ++j) { xn[j] = x[j]; gn[j] = g[j]; }
-        fn_val = f;
-      } else {
-        nfev += cvsrch<Fn, T, E, true, true>(fn, ctx, rc, x, f, g, xn, fn_val, gn, alpha_init, q, dginit);
-      }
+      lbfgs_search<LsMoreThuente>(fn, ctx, rc, x, f, g, xn, fn_val, gn, alpha_init, q, dginit, nfev);
 
       const T prev_value = f;
       T x_delta, gnorm_inf, x_inf;
@@ -414,39 +375,24 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
         T zd[E];
 #pragma unroll
         for (int j = 0; j < E; ++j) zd[j] = x[j] - x[j];
-        group_maxabs3<T, W>(rc, zd, g, x, x_delta, gnorm_inf, x_inf);
+        maxabs3(rc, zd, g, x, x_delta, gnorm_inf, x_inf);
       } else {
         // ---- pair + gamma update (:248-298) ----
         T sd[E], yd[E];
 #pragma unroll
         for (int j = 0; j < E; ++j) { sd[j] = xn[j] - x[j]; yd[j] = gn[j] - g[j]; }
-        T sy, ss, yy, xx_next;
-        warp_sum4_p<P, T, E>(lane_dot_p<P, T, E>(sd, yd), lane_dot_p<P, T, E>(sd, sd), lane_dot_p<P, T, E>(yd, yd),
-                             lane_dot_p<P, T, E>(xn, xn), rc, sy, ss, yy, xx_next);
-        if (uni(curvature_above_eps<T>(sy, ss, yy))) {  // :266
+        T sy, yy, xx_next;
+        if (uni(lbfgs_pair_sums<P>(rc, sd, yd, xn, sy, yy, xx_next))) {
           const T rho_new = T(1) / sy;
-          int slot = mem_count;
-          if (slot == M) {
-            slot = mem_pos;
-            mem_pos = (mem_pos + 1 == M) ? 0 : mem_pos + 1;
-          }
+          const int slot = hist.ring_slot();
           GV::store(S + slot * D, t, sd);
           GV::store(Yh + slot * D, t, yd);
           __syncwarp();  // all lanes are done reading rho_s in this iteration's loops
           if (lane == 0) rho_s[slot] = rho_new;
-          const unsigned usable = (cabs(sy) < eps) ? 0u : 1u;
-          if (mem_count < M) {
-            valid |= usable << mem_count;
-            mem_count++;
-          } else {
-            valid = (valid >> 1) | (usable << (M - 1));
-          }
+          hist.record(sy);
         }
-        if (yy > eps) {
-          const T temp_scaling = sy / yy;
-          if (cfinite(temp_scaling) && cabs(temp_scaling) <= T(1e7)) gamma = smax(temp_scaling, eps);
-        }
-        group_maxabs3<T, W>(rc, sd, gn, xn, x_delta, gnorm_inf, x_inf);
+        lbfgs_update_gamma(gamma, sy, yy);
+        maxabs3(rc, sd, gn, xn, x_delta, gnorm_inf, x_inf);
 #pragma unroll
         for (int j = 0; j < E; ++j) { x[j] = xn[j]; g[j] = gn[j]; }
         f = fn_val;

@@ -495,8 +495,8 @@ __device__ __forceinline__ int hzls(const Fn& fn, const EvalCtx& ctx, const RedC
 struct LsMoreThuente {
   // cvsrch always evaluates at the step it returns: the returned state IS x0 + stp * s
   static constexpr bool kStateMayDifferFromStep = false;
-  template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false>
-  __device__ __forceinline__ static int search(const Fn& fn, const EvalCtx& ctx, const RedCtx<T>& rc,
+  template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false, class RC>
+  __device__ __forceinline__ static int search(const Fn& fn, const EvalCtx& ctx, const RC& rc,
                                                const T (&x0)[E], const T f0, const T (&g0)[E], T (&x)[E],
                                                T& f, T (&g)[E], T stp, const T (&s)[E], const T dginit) {
     return cvsrch<Fn, T, E, kNeg, kChecked>(fn, ctx, rc, x0, f0, g0, x, f, g, stp, s, dginit);
