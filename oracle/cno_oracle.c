@@ -32,6 +32,7 @@ static inline int problem_lbfgs_m(const cno_problem_t* p) {
 #define R_FMAX fmax
 #define R_ISFINITE isfinite
 #define R_IS_F32 0
+#define R_MIN_NORMAL DBL_MIN
 #include "cno_oracle_impl.inc"
 #undef REAL
 #undef FN
@@ -42,6 +43,7 @@ static inline int problem_lbfgs_m(const cno_problem_t* p) {
 #undef R_FMAX
 #undef R_ISFINITE
 #undef R_IS_F32
+#undef R_MIN_NORMAL
 
 /* ---- float ---- */
 #define REAL float
@@ -53,6 +55,7 @@ static inline int problem_lbfgs_m(const cno_problem_t* p) {
 #define R_FMAX fmaxf
 #define R_ISFINITE isfinite
 #define R_IS_F32 1
+#define R_MIN_NORMAL FLT_MIN
 #include "cno_oracle_impl.inc"
 #undef REAL
 #undef FN
@@ -113,7 +116,7 @@ int cno_oracle_minimize(int solver, const cno_problem_t* problem, int64_t batch,
 
 static int minimize_batch(int solver, const cno_problem_t* problem, int64_t batch, const void* x0,
                           const cno_stop_t* stop, const cno_batch_out_t* out, int threads, int linesearch,
-                          cno_lbfgs_paths_t* paths) {
+                          void* paths) {
   int rc = check_problem(solver, problem);
   if (linesearch != CNO_LS_MORE_THUENTE && linesearch != CNO_LS_HAGER_ZHANG) return CNO_ERR_INVALID_ARGUMENT;
   if (linesearch == CNO_LS_HAGER_ZHANG && solver != CNO_LBFGS && solver != CNO_BFGS &&
@@ -135,6 +138,9 @@ static int minimize_batch(int solver, const cno_problem_t* problem, int64_t batc
 #endif
 #pragma omp parallel for schedule(dynamic, 1) num_threads(threads)
   for (int64_t b = 0; b < batch; ++b) {
+    void* const pb = !paths ? NULL
+                     : solver == CNO_BFGS ? (void*)((cno_bfgs_paths_t*)paths + b)
+                                          : (void*)((cno_lbfgs_paths_t*)paths + b);
     if (problem->dtype == CNO_F64) {
       minimize_one_f64(
           solver, problem, NULL, linesearch, b, (const double*)x0 + b * d, stop,
@@ -145,7 +151,7 @@ static int minimize_batch(int solver, const cno_problem_t* problem, int64_t batc
           out->status ? out->status + b : NULL, out->nfev ? out->nfev + b : NULL,
           out->x_delta ? (double*)out->x_delta + b : NULL,
           out->f_delta ? (double*)out->f_delta + b : NULL,
-          out->gradient_norm ? (double*)out->gradient_norm + b : NULL, paths ? paths + b : NULL);
+          out->gradient_norm ? (double*)out->gradient_norm + b : NULL, pb);
     } else {
       minimize_one_f32(
           solver, problem, NULL, linesearch, b, (const float*)x0 + b * d, stop,
@@ -156,7 +162,7 @@ static int minimize_batch(int solver, const cno_problem_t* problem, int64_t batc
           out->status ? out->status + b : NULL, out->nfev ? out->nfev + b : NULL,
           out->x_delta ? (float*)out->x_delta + b : NULL,
           out->f_delta ? (float*)out->f_delta + b : NULL,
-          out->gradient_norm ? (float*)out->gradient_norm + b : NULL, paths ? paths + b : NULL);
+          out->gradient_norm ? (float*)out->gradient_norm + b : NULL, pb);
     }
   }
   return CNO_OK;
@@ -174,6 +180,13 @@ int cno_oracle_lbfgs_paths(const cno_problem_t* problem, int64_t batch, const vo
   if (!paths) return CNO_ERR_INVALID_ARGUMENT;
   if (batch > 0) memset(paths, 0, sizeof(*paths) * (size_t)batch);
   return minimize_batch(CNO_LBFGS, problem, batch, x0, stop, out, threads, CNO_LS_MORE_THUENTE, paths);
+}
+
+int cno_oracle_bfgs_paths(const cno_problem_t* problem, int64_t batch, const void* x0, const cno_stop_t* stop,
+                          const cno_batch_out_t* out, cno_bfgs_paths_t* paths, int threads, int linesearch) {
+  if (!paths) return CNO_ERR_INVALID_ARGUMENT;
+  if (batch > 0) memset(paths, 0, sizeof(*paths) * (size_t)batch);
+  return minimize_batch(CNO_BFGS, problem, batch, x0, stop, out, threads, linesearch, paths);
 }
 
 int cno_oracle_evaluate(const cno_problem_t* problem, int64_t batch,

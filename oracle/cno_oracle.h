@@ -62,6 +62,27 @@ int cno_oracle_lbfgs_paths(const cno_problem_t* problem, int64_t batch, const vo
                            const cno_stop_t* stop, const cno_batch_out_t* out,
                            cno_lbfgs_paths_t* paths, int threads);
 
+/* How often one Bfgs instance took the rare branches of OptimizationStep (bfgs.h:73-137), so that tests can show
+ * which paths an input reaches.  Counting only reads the step's values; the arithmetic is the same with or without. */
+typedef struct cno_bfgs_paths {
+  /* resets of H to the identity (bfgs.h:88-92): phi > 0, phi NaN */
+  uint64_t reset_positive, reset_nan;
+  /* updates refused by the curvature test (bfgs.h:125) while H was the identity (fresh) / after an update */
+  uint64_t refused_fresh, refused_updated;
+  /* curvature tests that the device's square-root-free bound (s.y > 0, (s.y)^2 and (s.s)(y.y) finite, (s.y)^2
+   * normal and (s.y)^2 > 2 eps^2 (s.s)(y.y); csrc/cno_device.cuh: curvature_above_eps) does not decide, so the
+   * specification's expression does: by its outcome (false, true) */
+  uint64_t curvature_fallback[2];
+  /* line searches that returned a non-finite value */
+  uint64_t nonfinite;
+  /* fresh steps with ||d|| <= eps (alpha_init = 1, bfgs.h:100-106) */
+  uint64_t small_direction;
+} cno_bfgs_paths_t;
+
+/* cno_oracle_minimize_ls(CNO_BFGS, ...) that also fills paths[batch]. */
+int cno_oracle_bfgs_paths(const cno_problem_t* problem, int64_t batch, const void* x0, const cno_stop_t* stop,
+                          const cno_batch_out_t* out, cno_bfgs_paths_t* paths, int threads, int linesearch);
+
 /* HagerZhang<F,1>::Search on the 1-D quartic (((c4 v + c3) v + c2) v + c1) v + c0 of
  * src/test/hager_zhang_test.cc (Quadratic, Cubic, FlatQuartic) along s = +1 from x0. */
 int cno_oracle_hz_search_poly(const double coef[5], double x0, double alpha_init,

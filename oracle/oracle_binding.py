@@ -163,6 +163,27 @@ def lbfgs_paths(family: int, x0: np.ndarray, *, stop: Stop | None = None, lbfgs_
     return r, paths
 
 
+BFGS_PATHS = ("reset_positive", "reset_nan", "refused_fresh", "refused_updated", "curvature_fallback_false",
+              "curvature_fallback_true", "nonfinite", "small_direction")  # the fields of cno_bfgs_paths_t
+
+
+def bfgs_paths(family: int, x0: np.ndarray, *, stop: Stop | None = None, linesearch: int = LS_MORE_THUENTE,
+               policy: int | None = None, threads: int = 0) -> tuple[dict, dict]:
+    """minimize(BFGS, family, x0, linesearch=linesearch), plus how often each instance took the rare branches of
+    OptimizationStep (cno_bfgs_paths_t): one [B] count per name of BFGS_PATHS."""
+    x0 = np.ascontiguousarray(x0)
+    B, d = x0.shape
+    p = Problem(family, _np_dtype(x0), d, 0, 0.0, None, 0, device_policy(x0.dtype) if policy is None else policy, 0, 0)
+    r, o = _batch_out(x0)
+    raw = np.zeros((B, len(BFGS_PATHS)), np.uint64)
+    rc = oracle_lib().cno_oracle_bfgs_paths(C.byref(p), C.c_int64(B), C.c_void_p(x0.ctypes.data),
+                                            C.byref(stop) if stop is not None else None, C.byref(o),
+                                            C.c_void_p(raw.ctypes.data), threads, linesearch)
+    if rc != 0:
+        raise RuntimeError(f"oracle bfgs_paths failed: {rc}")
+    return r, {k: raw[:, i] for i, k in enumerate(BFGS_PATHS)}
+
+
 def evaluate(family: int, x: np.ndarray, *, policy: int | None = None, data=None, n: int = 0,
              param: float = 0.0, hessian: bool = False):
     x = np.ascontiguousarray(x)
