@@ -12,6 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcno.so")
+USER_GROUP_PARTS = 5  # translation units of tests/cpp/user_group_functions.cu (CNO_USER_GROUP_PART)
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -89,9 +90,18 @@ def build_cpp_tests(verbose: bool = False) -> list:
         if current(source, target):
             continue
         procs.append(subprocess.Popen([nvcc, *dev_flags, *extra, source, *inc, "-o", target, f"-L{HERE}", "-lcno", *xlink]))
+    # user functors and composites at d = 512 / 1024 (tests/test_user_group_gpu.py): compiled in parts, in parallel
+    group_src, group_lib = os.path.join(src, "user_group_functions.cu"), os.path.join(out, "libcno_usergroup.so")
+    group_objs = [os.path.join(out, f"user_group_functions.{k}.o") for k in range(USER_GROUP_PARTS)]
+    if not current(group_src, group_lib):
+        procs += [subprocess.Popen([nvcc, *dev_flags, "-c", "-Xcompiler", "-fPIC", f"-DCNO_USER_GROUP_PART={k}",
+                                    group_src, *inc, "-o", obj]) for k, obj in enumerate(group_objs)]
     for p in procs:
         if p.wait() != 0:
             raise subprocess.CalledProcessError(p.returncode, p.args)
+    if not current(group_src, group_lib):
+        subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", *group_objs, "-o", group_lib,
+                        f"-L{HERE}", "-lcno", *xlink], check=True)
     exes.append(os.path.join(out, "user_functor"))
     return exes
 

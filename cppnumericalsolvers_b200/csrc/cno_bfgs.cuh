@@ -165,14 +165,20 @@ bfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
 // E elements per lane.  Same arithmetic specification as the register-resident kernel: (Hv)_i = sum_j H_ij
 // v_j, j ascending from the first product; H_ij = (H_ij - rho (s_i Hy_j + Hy_i s_j)) + c2 (s_i s_j).
 // One instance needs 8 D^2 bytes (32 KB at d = 64 fp64: 6 resident warps per SM; 128 KB at d = 128: one).
+// The slice of one warp apart from the plan, so that BfgsPlan::kFits can ask whether it fits without the plan's check.
 template <class T, int D>
-struct BfgsBigSmem {
+struct BfgsBigSlice {
   static constexpr int E = Shape<D>::E;
   static constexpr int kRows = 32 * E;  // padded rows of a column
   static constexpr int kH = D * kRows;
   static constexpr int kWarpElems = ((kH + 2 * kRows + CNO_MAX_PAST + 3) / 4) * 4;
   static constexpr size_t kWarpBytes = (size_t)kWarpElems * sizeof(T);
   static constexpr int kFit = (int)((size_t)(227 * 1024) / kWarpBytes);
+};
+template <class T, int D>
+struct BfgsBigSmem : BfgsBigSlice<T, D> {
+  static constexpr int kFit = BfgsBigSlice<T, D>::kFit;
+  static constexpr size_t kWarpBytes = BfgsBigSlice<T, D>::kWarpBytes;
   static_assert(kFit >= 1, "BFGS: the inverse Hessian does not fit one SM's shared memory");
   static constexpr int kWarps = kFit > 8 ? 8 : kFit;
   static constexpr int kThreads = kWarps * 32;
@@ -334,14 +340,16 @@ bfgs_smem_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x
 }
 
 // The kernel of Bfgs<Fn> with line search LS and its plan: the inverse Hessian in registers for D <= 32, in shared
-// memory above.
+// memory above.  kFits: one instance's inverse Hessian fits one SM (false past d = 128 in fp64).
 template <class Fn, class LS, bool kBig = (Fn::Dim > 32)>
 struct BfgsPlan {
+  static constexpr bool kFits = true;
   using SM = BfgsSmem<typename Fn::Scalar, Fn::Dim>;
   static auto kernel() { return bfgs_minimize_kernel<Fn, LS>; }
 };
 template <class Fn, class LS>
 struct BfgsPlan<Fn, LS, true> {
+  static constexpr bool kFits = BfgsBigSlice<typename Fn::Scalar, Fn::Dim>::kFit >= 1;
   using SM = BfgsBigSmem<typename Fn::Scalar, Fn::Dim>;
   static auto kernel() { return bfgs_smem_minimize_kernel<Fn, LS>; }
 };

@@ -21,6 +21,18 @@
 //   kHelperWarps = 1 + helper()/release_helper()   a second warp per instance that the functor drives through a
 //                                       named barrier (FnHelperWarps; LogisticFn, built-in functors only)
 //
+// Group form (fp64, First mode; HasGroupForm): a second operator() for the group L-BFGS kernel (cno_lbfgs_group.cuh),
+// in which W = d / 128 warps own one instance:
+//     __device__ double operator()(const cno::GroupEvalCtx<W>& c, const double (&x)[4], double (*grad)[4]) const;
+//   thread t = 32 w + l of the group holds elements c.first .. c.first + 3 (c.first = group_first_elem<W>(t): lane l's
+//   run of d / 32 elements, warp w's 4 of them); returns f(x) in every thread and, if grad != nullptr, the thread's 4
+//   gradient elements.  The functor never writes a barrier: group_sum_terms(c, terms) sums 4 terms per thread over the
+//   group with the bits of warp_sum(lane_tree<T, d / 32>(terms)) in the one-warp form; group_neighbours(c, x, x_prev,
+//   x_next) gives x_{first-1} and x_{first+4} through the group's exchange block.  Barrier rule: an evaluation that
+//   uses the exchange block is followed by a group sum before the block is written again (a functor that returns
+//   group_sum_terms keeps it, and so does every composite of such functors).  CNO_INSTANTIATE_FUNCTION runs Lbfgs
+//   (MoreThuente, default policy, nothing staged) on this form at d = 1024.
+//
 // The operation order of each functor below is restated one-for-one by the
 // CPU oracle (oracle/cno_oracle_impl.inc: eval_*), so values and gradients
 // agree bit for bit.

@@ -152,8 +152,8 @@ __device__ __forceinline__ T lbfgs_direction(const RC& rc, const T (&g)[E], T (&
 
 // MoreThuente::Search / HagerZhang (lbfgs.h:231-232) along -q, its evaluations added to nfev, or the search's own
 // early return for dginit >= 0 (more_thuente.h:152-156): the state untouched.
-template <class LS, class Fn, class T, int E, class RC>
-__device__ __forceinline__ void lbfgs_search(const Fn& fn, const EvalCtx& ctx, const RC& rc, const T (&x)[E],
+template <class LS, class Fn, class T, int E, class Ctx, class RC>
+__device__ __forceinline__ void lbfgs_search(const Fn& fn, const Ctx& ctx, const RC& rc, const T (&x)[E],
                                              const T f, const T (&g)[E], T (&xn)[E], T& fn_val, T (&gn)[E],
                                              const T alpha_init, const T (&q)[E], const T dginit, uint32_t& nfev) {
   if (uni(dginit >= T(0))) {

@@ -19,8 +19,11 @@
 // lbfgs_pair_sums, lbfgs_update_gamma, maxabs3) on a GroupCtx, with the whole history in shared memory (R = 0); the two
 // loops of the recursion and the pair store are the group's own.
 //
-// Not covered: user functors (a block-cooperative functor concept is a public-interface change), register-held pairs,
-// the stepwise (parked) form, Second mode, HagerZhang.
+// Functors: the built-in GroupRosenbrockFn, and any fp64 functor with the group form of the functor concept
+// (cno_functors.cuh; GroupEvalCtx, group_sum_terms, group_neighbours below).  CNO_INSTANTIATE_FUNCTION routes Lbfgs on
+// such a functor here at d = 1024 (include/cppoptlib_b200/device.cuh: user_minimize).
+//
+// Not covered: register-held pairs, the stepwise (parked) form, Second mode, HagerZhang, staged functors (kStageElems).
 #ifndef CNO_LBFGS_GROUP_CUH_
 #define CNO_LBFGS_GROUP_CUH_
 
@@ -103,6 +106,41 @@ __device__ __forceinline__ void warp_sum4_p(const typename LanePartial<P, T, E>:
   warp_sum4(ra, rb, rc_out, rd);
 }
 
+// ---- the group form of the functor concept (cno_functors.cuh): what a functor needs, so that it never writes a barrier
+// The first of thread t's 4 elements in a group of W warps (d = 128 W): lane l's run of d / 32 elements starts at
+// l d / 32, and warp w holds its 4 elements from 4 w on.
+template <int W>
+__device__ __forceinline__ int group_first_elem(int t) { return (t & 31) * (4 * W) + 4 * (t >> 5); }
+
+// The sum over the group of the functor's terms (4 per thread), in the order of the reduction specification (DESIGN.md
+// 3): the same bits as warp_sum(lane_tree<T, d / 32>(terms)) of the one-warp form.  Every thread gets the sum.  The sum
+// ends with a barrier of the whole group, and it flips the kernel's own double buffer (c.rc).
+template <int W>
+__device__ __forceinline__ double group_sum_terms(const GroupEvalCtx<W>& c, const double (&terms)[4]) {
+  double t[4] = {terms[0], terms[1], terms[2], terms[3]};
+  return warp_sum_p<PolicyFast, double, 4>(lane_tree<double, 4>(t), *c.rc);
+}
+
+// x_{first - 1} and x_{first + 4}, the neighbours of a thread's 4 elements, through the group's exchange block.  They
+// come from (w -+ 1, l), or at the ends of a lane's run from (W - 1, l - 1) and (0, l + 1).  At the ends of the vector
+// (x_{-1}, x_d) the thread gets its own x[3] and x[0]; those values are not elements and must not be used.
+// Barrier rule: an evaluation that calls this must be followed by a group sum (group_sum_terms, or the kernel's sum of
+// a partial) before the exchange block is written again -- every thread has then read its neighbours.  A functor that
+// returns group_sum_terms keeps the rule, so composites with several such leaves do too.
+template <int W, class T>
+__device__ __forceinline__ void group_neighbours(const GroupEvalCtx<W>& c, const T (&x)[4], T& x_prev, T& x_next) {
+  constexpr int NT = 32 * W;
+  const int t = c.lane, w = t >> 5, l = t & 31;
+  T* const xch = static_cast<T*>(c.stage);
+  xch[t] = x[0];
+  xch[NT + t] = x[3];
+  group_bar(c.team, NT);
+  const int tn = (w + 1 < W) ? t + 32 : (l + 1 < 32 ? l + 1 : t);        // owner of element first + 4
+  const int tp = (w > 0) ? t - 32 : (l > 0 ? 32 * (W - 1) + l - 1 : t);  // owner of element first - 1
+  x_next = xch[tn];
+  x_prev = xch[NT + tp];
+}
+
 // lpNorm<Infinity> of three group-distributed vectors in one barrier (warp_maxabs's specification: the largest IEEE bit
 // pattern of |v_i| read as an unsigned integer; order free): each warp's maximum, then the maximum over the W warps as
 // 64-bit patterns.
@@ -174,12 +212,10 @@ __device__ __forceinline__ void store_quad(T* __restrict__ p, const T (&v)[4]) {
   for (int c = 0; c < LP::NC; ++c) q[c] = LP::P::make(&v[c * LP::CE]);
 }
 
-// Chained Rosenbrock for a group (same operation order as RosenbrockFn and the oracle's eval_rosenbrock).  ctx.lane is
-// the thread's index t = 32 w + l in its group, ctx.stage the group's exchange block (2 x 32 W values), ctx.team the
-// group's named barrier.  x_{i+1} of a thread's last element and x_{i-1} of its first come from (w +- 1, l), or at the
-// ends of a lane's run from (0, l + 1) and (W - 1, l - 1); B_{i-1} = 200 (x_i - x_{i-1}^2) is then formed in the
-// thread that needs it (the same operands in the same order as in the thread that owns element i - 1).  The exchange
-// block is written again only at the next evaluation, after the barrier of the sum that follows every evaluation.
+// Chained Rosenbrock for a group (same operation order as RosenbrockFn and the oracle's eval_rosenbrock).  x_{i+1} of a
+// thread's last element and x_{i-1} of its first come from group_neighbours; B_{i-1} = 200 (x_i - x_{i-1}^2) is then
+// formed in the thread that needs it (the same operands in the same order as in the thread that owns element i - 1).
+// partial() leaves the sum to its caller, which keeps group_neighbours' barrier rule by summing it.
 template <class T, int D>
 struct GroupRosenbrockFn {
   static_assert(D % 128 == 0 && (D / 128 & (D / 128 - 1)) == 0 && D / 128 >= 2 && D / 128 <= 8,
@@ -194,20 +230,12 @@ struct GroupRosenbrockFn {
   static constexpr int kXchElems = 2 * 32 * kGroupWarps;
 
   // the first of thread t's 4 elements
-  __device__ __forceinline__ static int first_elem(int t) { return (t & 31) * (D / 32) + 4 * (t >> 5); }
+  __device__ __forceinline__ static int first_elem(int t) { return group_first_elem<kGroupWarps>(t); }
 
-  __device__ __forceinline__ T partial(const EvalCtx& c, const T (&x)[4], T (*grad)[4]) const {
-    constexpr int W = kGroupWarps, NT = 32 * W;
-    const int t = c.lane, w = t >> 5, l = t & 31;
-    T* const xch = static_cast<T*>(c.stage);
-    xch[t] = x[0];
-    xch[NT + t] = x[3];
-    group_bar(c.team, NT);
-    const int tn = (w + 1 < W) ? t + 32 : (l + 1 < 32 ? l + 1 : t);              // owner of element i0 + 4
-    const int tp = (w > 0) ? t - 32 : (l > 0 ? 32 * (W - 1) + l - 1 : t);        // owner of element i0 - 1
-    const T x_next = xch[tn];
-    const T x_prev = xch[NT + tp];
-    const int i0 = first_elem(t);
+  __device__ __forceinline__ T partial(const GroupEvalCtx<kGroupWarps>& c, const T (&x)[4], T (*grad)[4]) const {
+    T x_prev, x_next;
+    group_neighbours(c, x, x_prev, x_next);
+    const int i0 = c.first;
     T term[4], A[4], Bv[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -236,11 +264,30 @@ struct GroupRosenbrockFn {
     }
     return lane_tree<T, 4>(term);
   }
+  // the group form of the functor concept: the value summed over the group (what the mirror's Rosenbrock forwards to)
+  __device__ __forceinline__ T operator()(const GroupEvalCtx<kGroupWarps>& c, const T (&x)[4], T (*grad)[4]) const {
+    return warp_sum_p<PolicyFast, T, 4>(partial(c, x, grad), *c.rc);
+  }
+};
+
+// 0.5 * x.squaredNorm() for a group: HalfSquaredNormFn's arithmetic, summed over the group.
+template <int D>
+struct GroupHalfSquaredNormFn {
+  __device__ __forceinline__ double operator()(const GroupEvalCtx<D / 128>& c, const double (&x)[4],
+                                               double (*grad)[4]) const {
+    double t[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (grad) (*grad)[j] = x[j];
+      t[j] = x[j] * x[j];
+    }
+    return 0.5 * group_sum_terms(c, t);
+  }
 };
 
 // Shared memory of one group, in elements: history S[M][D], Y[M][D]; the double-buffered reduction scratch; the
 // functor's exchange block; the claimed instance id (16 bytes); then per warp rho[M], alpha[M] and the past-f ring.
-// Groups per CTA: as many as fit in 227 KB (at most 15: named barriers 1..15).
+// Groups per CTA: as many as fit in 227 KB (at most 15: named barriers 1..15); kFit = 0 when one group does not fit.
 template <class T, int D, int M>
 struct LbfgsGroupPlan {
   static constexpr int kGroupWarps = D / 128;
@@ -259,14 +306,14 @@ struct LbfgsGroupPlan {
   static constexpr int kMaxSmem = 227 * 1024;
   static constexpr int kFit = (int)(kMaxSmem / kGroupBytes);
   static constexpr int kGroups = kFit > 15 ? 15 : (kFit < 1 ? 1 : kFit);
-  static_assert(kFit >= 1, "one group's history does not fit in shared memory");
   // launch_persistent's plan: kWarps = resident instances per CTA (one per group), kThreads = the block
   static constexpr int kWarps = kGroups;
   static constexpr int kThreads = kGroups * kGroupThreads;
   static constexpr size_t kBytes = kGroupBytes * kGroups;
 };
 
-// Lbfgs<Fn, M>::Minimize with MoreThuente, First mode, on a group functor.
+// Lbfgs<Fn, M>::Minimize with MoreThuente, First mode, on a group functor: GroupRosenbrockFn (its unreduced partial,
+// reduced with ||x||^2 and the slopes) or a functor with the group form (it reduces its own value).
 template <class Fn, int M>
 __global__ void __launch_bounds__(LbfgsGroupPlan<typename Fn::Scalar, Fn::Dim, M>::kThreads, 1)
 lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, const long long batch,
@@ -275,6 +322,7 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
   using T = typename Fn::Scalar;
   constexpr int D = Fn::Dim;
   using PL = LbfgsGroupPlan<T, D, M>;
+  static_assert(PL::kFit >= 1, "one group's history does not fit in shared memory");
   constexpr int W = PL::kGroupWarps;
   constexpr int NT = PL::kGroupThreads;
   constexpr int E = 4;
@@ -293,7 +341,7 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
   T* const alpha = rho_s + M;
   T* const ring = alpha + M;
   const GroupCtx<T, W> rc{G + PL::kOffScratch, lane, warp, 1 + group, 0};
-  const int e0 = Fn::first_elem(t);
+  const int e0 = group_first_elem<W>(t);
 
   for (;;) {
     // ---- retire + refill: one thread of the group claims the next instance ----
@@ -301,7 +349,7 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
     group_bar(rc.bar, NT);
     const unsigned long long b = *claim;
     if (uni(b >= (unsigned long long)batch)) break;
-    const EvalCtx ctx{t, (long long)b, G + PL::kOffXch, rc.bar};
+    const GroupEvalCtx<W> ctx{t, (long long)b, G + PL::kOffXch, rc.bar, e0, &rc};
 
     T x[E], g[E];
     T f;
@@ -314,7 +362,12 @@ lbfgs_group_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__
     progress_start(prog);
     // ---- solver.h:189-192: evaluate once at the start point; ||x||^2 of lbfgs.h:95 in the same round ----
     load_quad<T, true>(x0 + b * D + e0, x);
-    warp_sum2_p<P, T, E>(fn.partial(ctx, x, &g), lane_dot_p<P, T, E>(x, x), rc, f, xx);
+    if constexpr (FnHasPartial<Fn>::value) {
+      warp_sum2_p<P, T, E>(fn.partial(ctx, x, &g), lane_dot_p<P, T, E>(x, x), rc, f, xx);
+    } else {
+      f = fn(ctx, x, &g);
+      xx = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(x, x), rc);
+    }
     nfev = 1;
 
     do {  // solver.h:196-220

@@ -146,9 +146,10 @@ __device__ __forceinline__ typename LanePartial<P, T, E>::type ls_dir_dot(const 
 // f(x0 +- stp*s) and g.(+-s): the trial point of every line search (more_thuente.h:198-201,
 // hager_zhang.h:152-159), f and the slope reduced together when the functor exposes its partial.
 // RC: the reduction context -- RedCtx<T> of the one-warp kernels, or the group context of a kernel in which several
-// warps share one instance (cno_lbfgs_group.cuh); warp_sum_p / warp_sum2_p are overloaded on it.
-template <bool kNeg, class Fn, class T, int E, class RC>
-__device__ __forceinline__ void ls_eval(const Fn& fn, const EvalCtx& ctx, const RC& rc, const T (&x0)[E],
+// warps share one instance (cno_lbfgs_group.cuh); warp_sum_p / warp_sum2_p are overloaded on it.  Ctx: the context
+// the functor is called with -- EvalCtx, or GroupEvalCtx<W> in the group kernel.
+template <bool kNeg, class Fn, class T, int E, class Ctx, class RC>
+__device__ __forceinline__ void ls_eval(const Fn& fn, const Ctx& ctx, const RC& rc, const T (&x0)[E],
                                         const T stp, const T (&s)[E], T (&x)[E], T& f, T (&g)[E], T& dg) {
   using P = typename PolicyOf<Fn>::type;
 #pragma unroll
@@ -162,8 +163,8 @@ __device__ __forceinline__ void ls_eval(const Fn& fn, const EvalCtx& ctx, const 
   }
 }
 
-template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false, class RC>
-__device__ __forceinline__ int cvsrch(const Fn& fn, const EvalCtx& ctx, const RC& rc, const T (&x0)[E],
+template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false, class Ctx, class RC>
+__device__ __forceinline__ int cvsrch(const Fn& fn, const Ctx& ctx, const RC& rc, const T (&x0)[E],
                                       const T f0, const T (&g0)[E], T (&x)[E], T& f,
                                       T (&g)[E], T stp, const T (&s)[E], const T dginit) {
   int info = 0;
@@ -495,8 +496,8 @@ __device__ __forceinline__ int hzls(const Fn& fn, const EvalCtx& ctx, const RedC
 struct LsMoreThuente {
   // cvsrch always evaluates at the step it returns: the returned state IS x0 + stp * s
   static constexpr bool kStateMayDifferFromStep = false;
-  template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false, class RC>
-  __device__ __forceinline__ static int search(const Fn& fn, const EvalCtx& ctx, const RC& rc,
+  template <class Fn, class T, int E, bool kNeg = false, bool kChecked = false, class Ctx, class RC>
+  __device__ __forceinline__ static int search(const Fn& fn, const Ctx& ctx, const RC& rc,
                                                const T (&x0)[E], const T f0, const T (&g0)[E], T (&x)[E],
                                                T& f, T (&g)[E], T stp, const T (&s)[E], const T dginit) {
     return cvsrch<Fn, T, E, kNeg, kChecked>(fn, ctx, rc, x0, f0, g0, x, f, g, stp, s, dginit);

@@ -262,12 +262,23 @@ struct BatchedFunctionState {
                                            bool transposed, typename DeviceFn::Scalar (&col)[E]) const {          \
     DeviceFn{}.hess_col(c, x, j, transposed, col);                                                                \
   }
+// The group form (cno_functors.cuh) of the fp64 families at d = 256, 512 and 1024: W = d / 128 warps per instance;
+// the functors of csrc/cno_lbfgs_group.cuh.
+#define CNO_BUILTIN_GROUP_FORM(...)                                                                               \
+  template <int W, class S = T, class = std::enable_if_t<std::is_same<S, double>::value && 128 * W == D &&         \
+                                                         (W == 2 || W == 4 || W == 8)>>                           \
+  __device__ __forceinline__ double operator()(const cno::GroupEvalCtx<W>& c, const double (&x)[4],               \
+                                               double (*grad)[4]) const {                                          \
+    return __VA_ARGS__{}(c, x, grad);                                                                              \
+  }
 #else
 #define CNO_BUILTIN_DEVICE_MEMBERS(...)
+#define CNO_BUILTIN_GROUP_FORM(...)
 #endif
 template <class T, int D>
 struct Rosenbrock : FunctionCRTP<Rosenbrock<T, D>, T, DifferentiabilityMode::First, D> {
   CNO_BUILTIN_DEVICE_MEMBERS(cno::RosenbrockFn<T, D>)
+  CNO_BUILTIN_GROUP_FORM(cno::GroupRosenbrockFn<double, D>)
 };
 template <class T, int D>
 struct RosenbrockFull : FunctionCRTP<RosenbrockFull<T, D>, T, DifferentiabilityMode::Second, D> {
@@ -280,6 +291,7 @@ struct DiagQuadratic : FunctionCRTP<DiagQuadratic<T>, T, DifferentiabilityMode::
 template <class T, int D>
 struct HalfSquaredNorm : FunctionCRTP<HalfSquaredNorm<T, D>, T, DifferentiabilityMode::First, D> {
   CNO_BUILTIN_DEVICE_MEMBERS(cno::HalfSquaredNormFn<T, D>)
+  CNO_BUILTIN_GROUP_FORM(cno::GroupHalfSquaredNormFn<D>)
 };
 // The Second-mode twins of the two families above (function_base.h:96-126 with Mode = Second), for
 // composites that need Hessians (NewtonDescent, Lbfgs's preconditioner branch).

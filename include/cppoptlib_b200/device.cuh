@@ -16,6 +16,17 @@
 //   CNO_DECLARE_FUNCTION(myf, MyF)        // host side: binds MyF to the symbols
 //   CNO_INSTANTIATE_FUNCTION(myf, MyF)    // device side: defines the symbols
 //
+// Any Dim compiles.  A solver whose plan does not fit one SM for it (in fp64: Bfgs past d = 128, NewtonDescent past
+// d = 169, the condition number past d = 120) returns CNO_ERR_UNSUPPORTED at run time; Lbfgs runs at every d.
+//
+// At d = 1024 (fp64) a functor may also have the group form of the functor concept (cno_functors.cuh), which the
+// mirror's Rosenbrock and HalfSquaredNorm and every composite of group-form functors have:
+//     __device__ double operator()(const cno::GroupEvalCtx<8>& c, const double (&x)[4], double (*grad)[4]) const;
+// with the helpers cno::group_sum_terms, cno::group_neighbours and cno::group_first_elem (cno_lbfgs_group.cuh).  Lbfgs
+// (MoreThuente, First mode, the default policy, nothing staged) on such a functor then runs the group kernel, d / 128
+// warps per instance, which was measured faster there than the one-warp kernel (DESIGN.md 2.10); every other case
+// runs the one-warp kernel as before.
+//
 // This is the "thin extern-C layer": one symbol set per instantiated functor (SURVEY.md 8(b)), behind
 // which Lbfgs / Bfgs / NewtonDescent / GradientDescent / ConjugatedGradientDescent<MyF>::Minimize,
 // SetCallback (stepwise solves) and FunctionExpr::operator() launch the same persistent kernels as the
@@ -42,6 +53,7 @@
 #endif
 #include "cno_device.cuh"
 #include "cno_functors.cuh"
+#include "cno_lbfgs_group.cuh"
 #define CPPOPTLIB_B200_WITH_DEVICE 1
 #include "cppoptlib.h"
 #include "expressions.h"
@@ -112,23 +124,37 @@ inline int user_lbfgs(const F& fn, int mode, int lbfgs_m, int64_t batch, const v
                                           workspace, workspace_bytes, stream, info, ResumeArgs{nullptr, 0, 0, 0});
 }
 
+// Lbfgs (MoreThuente) on the group kernel (cno_lbfgs_group.cuh) where it was measured faster than the one-warp kernel
+// (DESIGN.md 2.10): fp64 functors with the group form at d = 1024, the default policy, nothing staged, and m such that
+// one group's history fits one SM.  At d = 512 the one-warp kernel was faster; it keeps every other case.
+template <class F, int M>
+struct GroupLbfgsRoute {
+  static constexpr bool value = F::Dim == 1024 && std::is_same<typename F::Scalar, double>::value &&
+                                std::is_same<typename PolicyOf<F>::type, PolicyFast>::value &&
+                                StageElems<F>::value == 0 && HasGroupForm<F, F::Dim / 128>::value &&
+                                LbfgsGroupPlan<double, 1024, M>::kFit >= 1;
+};
+
 template <class F, class LS>
 inline int user_bfgs(const F& fn, int64_t batch, const void* x0, const cno_stop_t* stop, const cno_batch_out_t* out,
                      void* workspace, size_t workspace_bytes, void* stream, cno_launch_info_t* info) {
   using P = BfgsPlan<F, LS>;
-  return launch_user<F, typename P::SM>(P::kernel(), fn, batch, x0, stop, out, workspace, workspace_bytes, stream, info);
+  if constexpr (P::kFits)
+    return launch_user<F, typename P::SM>(P::kernel(), fn, batch, x0, stop, out, workspace, workspace_bytes, stream, info);
+  else
+    return CNO_ERR_UNSUPPORTED;  // the inverse Hessian does not fit one SM's shared memory
 }
 
 template <class F>
 inline int user_newton(const F& fn, int64_t batch, const void* x0, const cno_stop_t* stop, const cno_batch_out_t* out,
                        void* workspace, size_t workspace_bytes, void* stream, cno_launch_info_t* info) {
-  if constexpr (F::Mode == 2 && HasHessCol<F>::value) {
+  if constexpr (F::Mode == 2 && HasHessCol<F>::value && NewtonSmem<typename F::Scalar, F::Dim>::kWarpsFit >= 1) {
     using A = SecondOrderAdapter<F>;
     if (stop && stop->condition_hessian > 0) return CNO_ERR_UNSUPPORTED;
     return launch_user<A, NewtonSmem<typename F::Scalar, F::Dim>>(newton_minimize_kernel<A>, A{fn}, batch, x0, stop, out,
                                                                    workspace, workspace_bytes, stream, info);
   } else {
-    return CNO_ERR_UNSUPPORTED;  // NewtonDescent only supports second-order differentiable functions
+    return CNO_ERR_UNSUPPORTED;  // second-order differentiable functions whose Hessian fits one SM's shared memory
   }
 }
 
@@ -137,7 +163,7 @@ inline int user_newton(const F& fn, int64_t batch, const void* x0, const cno_sto
 template <class F>
 inline int user_condition(const F& fn, int64_t batch, const void* x, void* condition, void* workspace,
                           size_t workspace_bytes, void* stream) {
-  if constexpr (F::Mode == 2 && HasHessCol<F>::value) {
+  if constexpr (F::Mode == 2 && HasHessCol<F>::value && ConditionSmem<typename F::Scalar, F::Dim>::kWarpsFit >= 1) {
     using A = SecondOrderAdapter<F>;
     using T = typename F::Scalar;
     if (batch < 0) return CNO_ERR_INVALID_ARGUMENT;
@@ -153,7 +179,7 @@ inline int user_condition(const F& fn, int64_t batch, const void* x, void* condi
                                                        static_cast<const T*>(x), (long long)batch,
                                                        static_cast<T*>(condition), queue);
   } else {
-    return CNO_ERR_UNSUPPORTED;  // defined for second-order differentiable functions
+    return CNO_ERR_UNSUPPORTED;  // second-order differentiable functions whose Hessian fits one SM's shared memory
   }
 }
 
@@ -164,6 +190,13 @@ inline int user_minimize(int solver, int mode, int lbfgs_m, const F& fn, int64_t
   using T = typename F::Scalar;
   switch (solver) {
     case CNO_LBFGS:
+      if constexpr (GroupLbfgsRoute<F, M>::value) {
+        // First mode used: not Lbfgs's Second-mode preconditioner branch (user_lbfgs)
+        const bool second = F::Mode == 2 && HasHessDiag<F>::value && mode == 2;
+        if (!second && (lbfgs_m == 0 || lbfgs_m == M))
+          return launch_user<F, LbfgsGroupPlan<double, 1024, M>>(lbfgs_group_minimize_kernel<F, M>, fn, batch, x0, stop,
+                                                                 out, workspace, workspace_bytes, stream, info);
+      }
       return user_lbfgs<F, LsMoreThuente, M>(fn, mode, lbfgs_m, batch, x0, stop, out, workspace, workspace_bytes, stream, info);
     case CNO_LBFGS_HAGER_ZHANG:
       return user_lbfgs<F, LsHagerZhang, M>(fn, mode, lbfgs_m, batch, x0, stop, out, workspace, workspace_bytes, stream, info);

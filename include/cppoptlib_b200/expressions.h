@@ -35,6 +35,13 @@
 //        this lane's rows of column j of the Hessian -- or of ROW j when `transposed` (NewtonDescent's
 //        Armijo slope needs d'H, and a product's Hessian is not bitwise symmetric)
 // and every node composes them the way the reference composes hess_f / hess_g.
+//
+// Group form (fp64, First mode; cno_functors.cuh): a node has
+//   double operator()(const cno::GroupEvalCtx<W>&, const double (&x)[4], double (*grad)[4]) const
+// when all its children have it, with the same arithmetic as its one-warp operator() (both are eval() below).  A
+// composite of group-form leaves is then a group functor, which Lbfgs runs on the group kernel at d = 1024.  A node
+// itself takes no sum and touches no shared memory, so the barrier rule of the group form (cno_lbfgs_group.cuh:
+// group_neighbours) holds for a composite when it holds for each leaf.
 #ifndef CPPOPTLIB_B200_EXPRESSIONS_H_
 #define CPPOPTLIB_B200_EXPRESSIONS_H_
 
@@ -110,6 +117,10 @@ using cno::hess_col;
 using cno::hess_prepare;
 template <class T, int E>
 CNO_D T bcast_elem(const T (&v)[E], int j) { return cno::lane_bcast<T, E>(v, j); }
+
+// every operand has the group form of W warps
+template <int W, class... Fs>
+struct AllGroupForm : std::bool_constant<(cno::HasGroupForm<Fs, W>::value && ...)> {};
 #endif  // CNO_DEVICE_CODE
 }  // namespace expr_detail
 
@@ -122,7 +133,11 @@ struct ConstExpression : expr_detail::NodeBase<TScalar, TMode, TDimension> {
 #ifdef CNO_DEVICE_CODE
   using T = TScalar;
   static constexpr int E = Base::E;
-  CNO_D T operator()(const cno::EvalCtx&, const T (&)[E], T (*grad)[E]) const {
+  CNO_D T operator()(const cno::EvalCtx& ctx, const T (&x)[E], T (*grad)[E]) const { return eval(ctx, x, grad); }
+  template <int W>
+  CNO_D T operator()(const cno::GroupEvalCtx<W>& ctx, const T (&x)[4], T (*grad)[4]) const { return eval(ctx, x, grad); }
+  template <class Ctx, int N>
+  CNO_D T eval(const Ctx&, const T (&)[N], T (*grad)[N]) const {
     if (grad) expr_detail::set_zero(*grad);
     return c;
   }
@@ -144,13 +159,17 @@ struct AddExpression : expr_detail::NodeBase<typename F::ScalarType, TMode, F::D
 #ifdef CNO_DEVICE_CODE
   using T = typename F::ScalarType;
   static constexpr int E = Base::E;
-  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const {
-    T gg[E];
+  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const { return eval(c, x, grad); }
+  template <int W, class F_ = F, class G_ = G, class = std::enable_if_t<expr_detail::AllGroupForm<W, F_, G_>::value>>
+  CNO_D T operator()(const cno::GroupEvalCtx<W>& c, const T (&x)[4], T (*grad)[4]) const { return eval(c, x, grad); }
+  template <class Ctx, int N>
+  CNO_D T eval(const Ctx& c, const T (&x)[N], T (*grad)[N]) const {
+    T gg[N];
     const T fx_f = f(c, x, grad);
     const T fx_g = g(c, x, grad ? &gg : nullptr);
     if (grad) {
 #pragma unroll
-      for (int e = 0; e < E; ++e) (*grad)[e] = (*grad)[e] + gg[e];  // :117, :130
+      for (int e = 0; e < N; ++e) (*grad)[e] = (*grad)[e] + gg[e];  // :117, :130
     }
     return fx_f + fx_g;
   }
@@ -191,13 +210,17 @@ struct SubExpression : expr_detail::NodeBase<typename F::ScalarType, TMode, F::D
 #ifdef CNO_DEVICE_CODE
   using T = typename F::ScalarType;
   static constexpr int E = Base::E;
-  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const {
-    T gg[E];
+  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const { return eval(c, x, grad); }
+  template <int W, class F_ = F, class G_ = G, class = std::enable_if_t<expr_detail::AllGroupForm<W, F_, G_>::value>>
+  CNO_D T operator()(const cno::GroupEvalCtx<W>& c, const T (&x)[4], T (*grad)[4]) const { return eval(c, x, grad); }
+  template <class Ctx, int N>
+  CNO_D T eval(const Ctx& c, const T (&x)[N], T (*grad)[N]) const {
+    T gg[N];
     const T fx_f = f(c, x, grad);
     const T fx_g = g(c, x, grad ? &gg : nullptr);
     if (grad) {
 #pragma unroll
-      for (int e = 0; e < E; ++e) (*grad)[e] = (*grad)[e] - gg[e];  // :170, :183
+      for (int e = 0; e < N; ++e) (*grad)[e] = (*grad)[e] - gg[e];  // :170, :183
     }
     return fx_f - fx_g;
   }
@@ -237,7 +260,11 @@ struct MulExpression : expr_detail::NodeBase<TScalar, TMode, F::Dimension> {
 #ifdef CNO_DEVICE_CODE
   using T = TScalar;
   static constexpr int E = Base::E;
-  CNO_D T operator()(const cno::EvalCtx& ctx, const T (&x)[E], T (*grad)[E]) const {
+  CNO_D T operator()(const cno::EvalCtx& ctx, const T (&x)[E], T (*grad)[E]) const { return eval(ctx, x, grad); }
+  template <int W, class F_ = F, class = std::enable_if_t<expr_detail::AllGroupForm<W, F_>::value>>
+  CNO_D T operator()(const cno::GroupEvalCtx<W>& ctx, const T (&x)[4], T (*grad)[4]) const { return eval(ctx, x, grad); }
+  template <class Ctx, int N>
+  CNO_D T eval(const Ctx& ctx, const T (&x)[N], T (*grad)[N]) const {
     if (cno::uni(c == T(0))) {  // :219-227: the source is not evaluated (matters when it is not finite there)
       if (grad) expr_detail::set_zero(*grad);
       return T(0);
@@ -245,7 +272,7 @@ struct MulExpression : expr_detail::NodeBase<TScalar, TMode, F::Dimension> {
     const T fx = f(ctx, x, grad);
     if (grad) {
 #pragma unroll
-      for (int e = 0; e < E; ++e) (*grad)[e] = c * (*grad)[e];  // :235, :244
+      for (int e = 0; e < N; ++e) (*grad)[e] = c * (*grad)[e];  // :235, :244
       expr_detail::mask_pad<F::Dimension>(ctx.lane, *grad);
     }
     return c * fx;
@@ -284,13 +311,17 @@ struct ProdExpression : expr_detail::NodeBase<typename F::ScalarType, TMode, F::
 #ifdef CNO_DEVICE_CODE
   using T = typename F::ScalarType;
   static constexpr int E = Base::E;
-  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const {
-    T gg[E];
+  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const { return eval(c, x, grad); }
+  template <int W, class F_ = F, class G_ = G, class = std::enable_if_t<expr_detail::AllGroupForm<W, F_, G_>::value>>
+  CNO_D T operator()(const cno::GroupEvalCtx<W>& c, const T (&x)[4], T (*grad)[4]) const { return eval(c, x, grad); }
+  template <class Ctx, int N>
+  CNO_D T eval(const Ctx& c, const T (&x)[N], T (*grad)[N]) const {
+    T gg[N];
     const T fx = f(c, x, grad);
     const T gx = g(c, x, grad ? &gg : nullptr);
     if (grad) {
 #pragma unroll
-      for (int e = 0; e < E; ++e) (*grad)[e] = gx * (*grad)[e] + fx * gg[e];  // :291, :300 product rule
+      for (int e = 0; e < N; ++e) (*grad)[e] = gx * (*grad)[e] + fx * gg[e];  // :291, :300 product rule
       expr_detail::mask_pad<F::Dimension>(c.lane, *grad);
     }
     return fx * gx;
@@ -347,7 +378,11 @@ struct ZeroClampExpression : expr_detail::NodeBase<typename F::ScalarType, F::Di
   static constexpr int E = Base::E;
   // inactive <=> val >= 0 (MinZero :343) or val <= 0 (MaxZero :388); a NaN value is "active" in both
   CNO_D static bool inactive(T val) { return kMin ? (val >= T(0)) : (val <= T(0)); }
-  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const {
+  CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const { return eval(c, x, grad); }
+  template <int W, class F_ = F, class = std::enable_if_t<expr_detail::AllGroupForm<W, F_>::value>>
+  CNO_D T operator()(const cno::GroupEvalCtx<W>& c, const T (&x)[4], T (*grad)[4]) const { return eval(c, x, grad); }
+  template <class Ctx, int N>
+  CNO_D T eval(const Ctx& c, const T (&x)[N], T (*grad)[N]) const {
     const T val = f(c, x, grad);
     if (cno::uni(inactive(val))) {
       if (grad) expr_detail::set_zero(*grad);
@@ -396,6 +431,10 @@ struct ModeDowngrade : expr_detail::NodeBase<typename F::ScalarType, TargetMode,
   using T = typename F::ScalarType;
   static constexpr int E = Base::E;
   CNO_D T operator()(const cno::EvalCtx& c, const T (&x)[E], T (*grad)[E]) const {
+    return source(c, x, TargetMode == DifferentiabilityMode::None ? nullptr : grad);
+  }
+  template <int W, class F_ = F, class = std::enable_if_t<expr_detail::AllGroupForm<W, F_>::value>>
+  CNO_D T operator()(const cno::GroupEvalCtx<W>& c, const T (&x)[4], T (*grad)[4]) const {
     return source(c, x, TargetMode == DifferentiabilityMode::None ? nullptr : grad);
   }
 #endif
