@@ -19,6 +19,7 @@
 #include "cno_lbfgs.cuh"
 #include "cno_lbfgs_group.cuh"
 #include "cno_lbfgsb.cuh"
+#include "cno_lbfgsb_group.cuh"
 #include "cno_bfgs.cuh"
 #include "cno_descent.cuh"
 #include "cno_evaluate.cuh"
@@ -365,13 +366,24 @@ struct LbfgsbArgs {
   cudaStream_t stream;
   cno_launch_info_t* info;
 };
+template <class T>
+cno::BoundsArgs<T> bounds_args(const LbfgsbArgs& a) {
+  return cno::BoundsArgs<T>{a.bounds ? static_cast<const T*>(a.bounds->lower) : nullptr,
+                            a.bounds ? static_cast<const T*>(a.bounds->upper) : nullptr,
+                            a.bounds ? (long long)a.bounds->stride : 0};
+}
 template <class Fn, int M = 5>
 int lbfgsb(const Fn& fn, const LbfgsbArgs& a) {
   using T = typename Fn::Scalar;
-  const cno::BoundsArgs<T> bd{a.bounds ? static_cast<const T*>(a.bounds->lower) : nullptr,
-                              a.bounds ? static_cast<const T*>(a.bounds->upper) : nullptr,
-                              a.bounds ? (long long)a.bounds->stride : 0};
-  return launch_solve<cno::LbfgsbSmem<T, Fn::Dim, M>>(cno::lbfgsb_minimize_kernel<Fn, M>, fn, a, bd);
+  return launch_solve<cno::LbfgsbSmem<T, Fn::Dim, M>>(cno::lbfgsb_minimize_kernel<Fn, M>, fn, a, bounds_args<T>(a));
+}
+// d = 256 / 512 / 1024 fp64 (cno_lbfgsb_group.cuh): one group of d / 128 warps per instance, the history in the group's
+// shared memory; m = 5 and the default policy only.
+template <int D>
+int lbfgsb_group_rosenbrock(const LbfgsbArgs& a) {
+  using Fn = cno::GroupRosenbrockFn<double, D>;
+  return launch_solve<cno::LbfgsbGroupPlan<double, D, 5>>(cno::lbfgsb_group_minimize_kernel<Fn, 5>, Fn{}, a,
+                                                          bounds_args<double>(a));
 }
 template <class T, int D>
 int lbfgsb_rosenbrock(const LbfgsbArgs& a) { return lbfgsb(cno::RosenbrockFn<T, D>{}, a); }
@@ -398,6 +410,9 @@ const LbfgsbEntry kLbfgsbTable[] = {
     {CNO_FN_ROSENBROCK, CNO_F64, 37, lbfgsb_rosenbrock<double, 37>},
     {CNO_FN_ROSENBROCK, CNO_F64, 64, lbfgsb_rosenbrock<double, 64>},
     {CNO_FN_ROSENBROCK, CNO_F64, 128, lbfgsb_rosenbrock<double, 128>},
+    {CNO_FN_ROSENBROCK, CNO_F64, 256, lbfgsb_group_rosenbrock<256>},
+    {CNO_FN_ROSENBROCK, CNO_F64, 512, lbfgsb_group_rosenbrock<512>},
+    {CNO_FN_ROSENBROCK, CNO_F64, 1024, lbfgsb_group_rosenbrock<1024>},
     {CNO_FN_ROSENBROCK, CNO_F32, 37, lbfgsb_rosenbrock<float, 37>},
     {CNO_FN_DIAG_QUADRATIC, CNO_F64, 2, lbfgsb_diag_quadratic<double>},
     {CNO_FN_HALF_SQUARED_NORM, CNO_F64, 2, lbfgsb_half_sq_norm<double, 2>},

@@ -47,7 +47,7 @@ struct BoundsArgs {
 template <class T, int D, int M>
 struct LbfgsbSmem {
   static constexpr int E = Shape<D>::E;
-  static_assert(E <= 4, "Lbfgsb: d <= 128");
+  static_assert(E <= 4, "Lbfgsb: d <= 128 (d = 256, 512, 1024: cno_lbfgsb_group.cuh)");
   static constexpr int kVec = 32 * E;
   static constexpr int L2 = 2 * M;
   // Y[M][kVec] | S[M][kVec] | scratch[kVec] | MM[L2*L2] | NN[L2*L2] | SY[M*M] | SS[M*M] | ring[MAX_PAST] | piv (ints)
@@ -79,6 +79,94 @@ __device__ __forceinline__ int warp_argmin_pos(float v, int idx, bool has, float
   const int I = (int)__reduce_min_sync(kFullMask, (has && u == U) ? (unsigned)idx : 0xffffffffu);
   vmin = __uint_as_float(U);
   return I;
+}
+
+// ---- the 2k x 2k systems of the compact representation, on one warp (every warp of a group kernel holds its own
+// copy of the factors and runs the same code, so all copies hold the same bits) ----
+// (n x n) LU of a column-major matrix in shared memory (leading dimension LD): the shim's / Eigen's partial-pivot
+// elimination; pv[k] = the row exchanged with k at step k.
+template <int LD, class T>
+__device__ __forceinline__ void lu_factor_warp(T* A, int* pv, int n, int lane) {
+#pragma unroll 1
+  for (int k = 0; k < n; ++k) {
+    __syncwarp();
+    T best = cabs(A[k + k * LD]);
+    int p = k;
+#pragma unroll 1
+    for (int i = k + 1; i < n; ++i) {  // first maximal |a_ik| (uniform scan: n <= 2m)
+      const T v = cabs(A[i + k * LD]);
+      if (uni(v > best)) { best = v; p = i; }
+    }
+    if (lane == 0) pv[k] = p;
+    if (uni(p != k)) {
+      if (lane < n) {
+        const T a = A[k + lane * LD], b2 = A[p + lane * LD];
+        A[k + lane * LD] = b2;
+        A[p + lane * LD] = a;
+      }
+      __syncwarp();
+    }
+    const T pivot = A[k + k * LD];
+    const bool below = (lane > k) && (lane < n);
+    T lik = T(0);
+    if (below) {
+      lik = A[lane + k * LD] / pivot;
+      A[lane + k * LD] = lik;
+    }
+#pragma unroll 1
+    for (int j = k + 1; j < n; ++j) {
+      const T akj = A[k + j * LD];
+      if (below) A[lane + j * LD] = A[lane + j * LD] - lik * akj;
+    }
+  }
+  __syncwarp();
+}
+// solve with the factors: rhs entry i in lane i (i < n); returns the solution in the same convention
+template <int LD, class T>
+__device__ __forceinline__ T lu_solve_warp(const T* A, const int* pv, int n, T r, int lane) {
+#pragma unroll 1
+  for (int k = 0; k < n; ++k) {
+    const int p = pv[k];
+    if (uni(p != k)) {
+      const int src = (lane == k) ? p : ((lane == p) ? k : lane);
+      r = __shfl_sync(kFullMask, r, src);
+    }
+  }
+#pragma unroll 1
+  for (int k = 0; k < n; ++k) {
+    const T bk = __shfl_sync(kFullMask, r, k);
+    if (lane > k && lane < n) r = r - A[lane + k * LD] * bk;
+  }
+#pragma unroll 1
+  for (int k = n - 1; k >= 0; --k) {
+    const T akk = A[k + k * LD];
+    if (lane == k) r = r / akk;
+    const T xk = __shfl_sync(kFullMask, r, k);
+    if (lane < k) r = r - A[lane + k * LD] * xk;
+  }
+  return (lane < n) ? r : T(0);
+}
+
+// MM = [[D, L'], [L, theta S'S]] (column-major, leading dimension 2M) from the cached S'Y / S'S of the kp pairs, the
+// oldest in physical slot `base`: D = -1 * diag(S'Y) as a matrix (off-diagonal -0), L = strictly lower S'Y.
+template <int M, class T>
+__device__ __forceinline__ void mm_assemble_warp(T* MM, const T* SY, const T* SSc, const T theta, int kp, int base,
+                                                 int lane) {
+  constexpr int L2 = 2 * M;
+  auto slot = [&](int i) -> int { const int s2 = base + i; return s2 >= M ? s2 - M : s2; };
+  const int n = 2 * kp;
+  if (lane < n) {
+#pragma unroll 1
+    for (int j = 0; j < n; ++j) {
+      const int i = lane;
+      T v;
+      if (i < kp && j < kp) v = (i == j) ? (T(-1) * SY[slot(i) + slot(i) * M]) : (T(-1) * T(0));
+      else if (i < kp) v = (j - kp > i) ? SY[slot(j - kp) + slot(i) * M] : T(0);            // L'(i, j-kp) = L(j-kp, i)
+      else if (j < kp) v = (i - kp > j) ? SY[slot(i - kp) + slot(j) * M] : T(0);            // L(i-kp, j)
+      else v = SSc[slot(i - kp) + slot(j - kp) * M] * theta;
+      MM[i + j * L2] = v;
+    }
+  }
 }
 
 template <class Fn, int M = 5, class LS = LsMoreThuente>
@@ -119,67 +207,6 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
     for (int e = 0; e < E; ++e) base[lane * E + e] = v[e];
   };
   auto wdot = [&](const T (&a)[E], const T (&b)[E]) -> T { return warp_sum(lane_dot<T, E>(a, b)); };
-
-  // ---- (n x n) LU of a column-major matrix in shared memory: the shim's / Eigen's partial-pivot elimination ----
-  auto lu_factor = [&](T* A, int* pv, int n) {
-#pragma unroll 1
-    for (int k = 0; k < n; ++k) {
-      __syncwarp();
-      T best = cabs(A[k + k * L2]);
-      int p = k;
-#pragma unroll 1
-      for (int i = k + 1; i < n; ++i) {  // first maximal |a_ik| (uniform scan: n <= 10)
-        const T v = cabs(A[i + k * L2]);
-        if (uni(v > best)) { best = v; p = i; }
-      }
-      if (lane == 0) pv[k] = p;
-      if (uni(p != k)) {
-        if (lane < n) {
-          const T a = A[k + lane * L2], b2 = A[p + lane * L2];
-          A[k + lane * L2] = b2;
-          A[p + lane * L2] = a;
-        }
-        __syncwarp();
-      }
-      const T pivot = A[k + k * L2];
-      const bool below = (lane > k) && (lane < n);
-      T lik = T(0);
-      if (below) {
-        lik = A[lane + k * L2] / pivot;
-        A[lane + k * L2] = lik;
-      }
-#pragma unroll 1
-      for (int j = k + 1; j < n; ++j) {
-        const T akj = A[k + j * L2];
-        if (below) A[lane + j * L2] = A[lane + j * L2] - lik * akj;
-      }
-    }
-    __syncwarp();
-  };
-  // solve with the factors: rhs entry i in lane i (i < n); returns the solution in the same convention
-  auto lu_solve = [&](const T* A, const int* pv, int n, T r) -> T {
-#pragma unroll 1
-    for (int k = 0; k < n; ++k) {
-      const int p = pv[k];
-      if (uni(p != k)) {
-        const int src = (lane == k) ? p : ((lane == p) ? k : lane);
-        r = __shfl_sync(kFullMask, r, src);
-      }
-    }
-#pragma unroll 1
-    for (int k = 0; k < n; ++k) {
-      const T bk = __shfl_sync(kFullMask, r, k);
-      if (lane > k && lane < n) r = r - A[lane + k * L2] * bk;
-    }
-#pragma unroll 1
-    for (int k = n - 1; k >= 0; --k) {
-      const T akk = A[k + k * L2];
-      if (lane == k) r = r / akk;
-      const T xk = __shfl_sync(kFullMask, r, k);
-      if (lane < k) r = r - A[lane + k * L2] * xk;
-    }
-    return (lane < n) ? r : T(0);
-  };
 
   for (;;) {
     const unsigned long long b = claim_instance(queue, lane);
@@ -230,7 +257,7 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
       auto w_entry = [&](int row, int i) -> T {
         return (i < kp) ? Ys[slot(i) * kVec + row] : (theta * Ss[slot(i - kp) * kVec + row]);
       };
-      auto solveM = [&](T r) -> T { return (have_lu && n2 > 0) ? lu_solve(MM, piv, n2, r) : r; };  // :311-316
+      auto solveM = [&](T r) -> T { return (have_lu && n2 > 0) ? lu_solve_warp<L2>(MM, piv, n2, r, lane) : r; };  // :311-316
 
       // ---- :145-150 project the iterate; re-evaluate if it moved ----
       T xcur[E];
@@ -488,8 +515,8 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
             const T mn = solveM(ncol);
             if (lane < n2) NN[lane + j * L2] = ((lane == j) ? T(1) : T(0)) - mn;
           }
-          lu_factor(NN, pivN, n2);
-          vv = lu_solve(NN, pivN, n2, vv);
+          lu_factor_warp<L2>(NN, pivN, n2, lane);
+          vv = lu_solve_warp<L2>(NN, pivN, n2, vv, lane);
         }
         // du = -(1/theta) r - (1/theta)^2 (W'Z)' v   (:515-516); alpha* (:451-475); subspace_min (:520-524)
         T du[E];
@@ -581,6 +608,7 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
         }
         __syncwarp();
         // MM = [[D, L'], [L, theta S'S]], D = -1 * diag(S'Y) as a matrix (off-diagonal -0), L = strictly lower S'Y
+        // (mm_assemble_warp's arithmetic, written out here: calling it costs this kernel two to four registers)
         const int n = 2 * kp;
         if (lane < n) {
 #pragma unroll 1
@@ -594,7 +622,7 @@ lbfgsb_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0, 
             MM[i + j * L2] = v;
           }
         }
-        lu_factor(MM, piv, n);
+        lu_factor_warp<L2>(MM, piv, n, lane);
         have_lu = true;
       }
 

@@ -337,7 +337,9 @@ class Lbfgsb(Solver):
             _lib.lib().cno_lbfgsb_default_stop(C.byref(s))
             progress = Progress.from_c(s)
         super().__init__(progress)
-        self.m = int(m)  # Lbfgsb<F, m>: pairs kept (compiled: 5 for every built-in, 10 for Rosenbrock d = 8 / 37 / 128)
+        # Lbfgsb<F, m>: pairs kept (compiled: 5 for every built-in, 10 for Rosenbrock d = 8 / 37 / 128); Rosenbrock fp64
+        # at d = 256 / 512 / 1024 runs on the group kernel (m = 5)
+        self.m = int(m)
         self.lower_bound: Optional[torch.Tensor] = None
         self.upper_bound: Optional[torch.Tensor] = None
 

@@ -250,7 +250,9 @@ void cno_lbfgsb_default_stop(cno_stop_t* stop);
 /* 0 if a kernel is instantiated for Lbfgsb on this problem, else CNO_ERR_UNSUPPORTED. */
 int cno_lbfgsb_supported(const cno_problem_t* problem);
 /* Batched Lbfgsb::Minimize (:238-286: the projected-gradient sup-norm drives stop->gradient_norm).  Device
- * pointers; bounds may be NULL (unbounded); stop NULL = cno_lbfgsb_default_stop; workspace as for cno_minimize. */
+ * pointers; bounds may be NULL (unbounded); stop NULL = cno_lbfgsb_default_stop; workspace as for cno_minimize.
+ * Compiled: the built-in families up to d = 128 (one warp per instance), and Rosenbrock fp64 with m = 5 and the
+ * default policy at d = 256, 512 and 1024 (one group of d / 128 warps per instance). */
 int cno_lbfgsb_minimize(const cno_problem_t* problem, const cno_bounds_t* bounds, int64_t batch, const void* x0,
                         const cno_stop_t* stop, const cno_batch_out_t* out, void* workspace, size_t workspace_bytes,
                         void* stream, cno_launch_info_t* info);

@@ -720,7 +720,8 @@ class Lbfgs : public Solver<F, LineSearch::solver_id(CNO_LBFGS)> {
 };
 // solver/lbfgsb.h:44-538: Lbfgsb<F, m = 5, MoreThuente> -- L-BFGS-B (box constraints).  The constructor carries the
 // reference's preset (default + f_delta = 2.22e-9 relative, :78-81); SetBounds (:88-92) takes device arrays [d]
-// (one box for the batch) or [B, d].
+// (one box for the batch) or [B, d].  Compiled keys: the built-ins of cno_api.cu up to d = 128, Rosenbrock fp64 at m = 10
+// (d = 8, 37, 128), and Rosenbrock fp64 at m = 5 for d = 256, 512 and 1024 (one group of d / 128 warps per instance).
 template <class F, int m = 5>
 class Lbfgsb {
   static_assert(m == 5 || m == 10, "Lbfgsb<F, m>: kernels are compiled for m = 5 (every built-in) and m = 10 (Rosenbrock)");
