@@ -1187,4 +1187,17 @@ int cno_al_minimize(const cno_problem_t* objective, const cno_constraints_t* con
   return al_find(objective)->fn(objective, constraints, a);
 }
 
+#ifdef CNO_LBFGS_PHASE_CLOCKS
+// The phase probe's counters of lbfgs_minimize_kernel (cno_lbfgs.cuh), copied to out[0 .. n) and zeroed.  Only a
+// measurement build compiled with -DCNO_LBFGS_PHASE_CLOCKS has it (tools/lbfgs_phase_clocks.py).
+int cno_lbfgs_phase_clocks_take(unsigned long long* out, int n) {
+  if (n != cno::kPhSlots) return CNO_ERR_INVALID_ARGUMENT;
+  unsigned long long zero[cno::kPhSlots] = {};
+  if (cudaMemcpyFromSymbol(out, cno::cno_lbfgs_phase_clocks, sizeof(zero)) != cudaSuccess ||
+      cudaMemcpyToSymbol(cno::cno_lbfgs_phase_clocks, zero, sizeof(zero)) != cudaSuccess)
+    return CNO_ERR_CUDA;
+  return CNO_OK;
+}
+#endif
+
 }  // extern "C"

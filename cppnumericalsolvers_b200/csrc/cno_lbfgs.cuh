@@ -38,6 +38,82 @@
 
 namespace cno {
 
+// Phase clock probe of lbfgs_minimize_kernel.  tools/lbfgs_phase_clocks.py builds a copy of the library with
+// -DCNO_LBFGS_PHASE_CLOCKS; without it every member below is empty and the kernel compiles to the same code.  Lane 0
+// of each warp reads clock64() at the phase boundaries of each steady-state iteration (full history, every pair
+// usable, a line search run), adds the phase's cycles to per-warp counters and, when the warp exits, adds those into
+// cno_lbfgs_phase_clocks: the cycles of each phase, then the iterations counted, the evaluations past each search's
+// first trial, and the loop-backs counted (the loop-back phase runs from the end of one counted iteration to the
+// start of the next).
+enum LbfgsPhase {
+  kPhRecursion, kPhDirection, kPhFirstTrial, kPhMoreTrials, kPhPairUpdate, kPhProgress, kPhLoopBack,
+  kPhIterations, kPhExtraEvals, kPhLoopBacks, kPhSlots
+};
+#ifdef CNO_LBFGS_PHASE_CLOCKS
+__device__ unsigned long long cno_lbfgs_phase_clocks[kPhSlots];
+struct LbfgsPhaseProbe {
+  unsigned long long acc[kPhSlots];
+  long long t, cur[kPhLoopBack];
+  bool steady, counted;
+  __device__ __forceinline__ void init() {
+#pragma unroll
+    for (int i = 0; i < kPhSlots; ++i) acc[i] = 0;
+    counted = false;
+  }
+  __device__ __forceinline__ void top() {  // start of an iteration
+    const long long n = clock64();
+    if (counted) {
+      acc[kPhLoopBack] += n - t;
+      acc[kPhLoopBacks]++;
+    }
+    t = n;
+    steady = false;
+    counted = false;
+  }
+  __device__ __forceinline__ void set_steady() { steady = true; }
+  __device__ __forceinline__ void mark(const int phase) {  // end of `phase`
+    const long long n = clock64();
+    cur[phase] = n - t;
+    t = n;
+  }
+  __device__ __forceinline__ void search(const bool searched, const uint32_t evals) {  // end of the line search
+    const long long n = clock64(), first = cno_ls_first_trial_clock[threadIdx.x >> 5];
+    cur[kPhFirstTrial] = first - t;
+    cur[kPhMoreTrials] = n - first;
+    t = n;
+    steady = steady && searched;
+    if (steady) acc[kPhExtraEvals] += evals - 1;
+  }
+  __device__ __forceinline__ void end() {  // end of the iteration (Progress::Update done)
+    mark(kPhProgress);
+    if (steady) {
+#pragma unroll
+      for (int i = 0; i < kPhLoopBack; ++i) acc[i] += cur[i];
+      acc[kPhIterations]++;
+    }
+    counted = steady;
+  }
+  __device__ __forceinline__ void stop() { counted = false; }  // the instance is done: no loop-back
+  __device__ __forceinline__ void flush(const int lane) {
+    if (lane == 0) {
+#pragma unroll
+      for (int i = 0; i < kPhSlots; ++i) atomicAdd(&cno_lbfgs_phase_clocks[i], acc[i]);
+    }
+  }
+};
+#else
+struct LbfgsPhaseProbe {
+  __device__ __forceinline__ void init() {}
+  __device__ __forceinline__ void top() {}
+  __device__ __forceinline__ void set_steady() {}
+  __device__ __forceinline__ void mark(int) {}
+  __device__ __forceinline__ void search(bool, uint32_t) {}
+  __device__ __forceinline__ void end() {}
+  __device__ __forceinline__ void stop() {}
+  __device__ __forceinline__ void flush(int) {}
+};
+#endif
+
 // The warp's shared-memory slice when the kRegPairs newest (s, y) pairs are held in registers and the older
 // M - kRegPairs in shared memory.
 template <class T, int D, int M, int kStage = 0, int kScratchPerLane = 0, int kMaxW = 16, int kHelpers = 0,
@@ -301,6 +377,8 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
     if (solver_warp) fn.init_stage(EvalCtx{lane, 0, stage_ptr, slot});
   }
 
+  LbfgsPhaseProbe probe;
+  probe.init();
   for (; solver_warp;) {
     // ---- retire + refill: next instance from the global queue ----
     const unsigned long long b = claim_instance(queue, lane);
@@ -370,8 +448,10 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       xx = warp_sum_p<P, T, E>(lane_dot_p<P, T, E>(x, x), rc);
     }
     int local_it = 0;
+    const auto max_local_it = ra.max_iterations;  // (`ra` is shadowed inside the loop)
 
-    do {  // solver.h:196-220
+    for (;;) {  // solver.h:196-220
+      probe.top();
       // ================= Lbfgs::OptimizationStep (lbfgs.h:89-303) =========
       // Second mode (:129-135): M^-1 = 1 / (|diag H| + eps); the gradient the reference
       // re-evaluates there is the state's gradient (same function, same x, same bits).
@@ -392,9 +472,11 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       // loop 2 the reverse.  In both loops the loads of the next shared pair are issued before the current
       // reduction (the reduction is the critical path; LDS latency hides under it).
       T ra[RA];  // alpha of the register pairs
-      if (uni(k == M && hist.valid == ((1u << M) - 1u))) {
+      const bool full = uni(k == M && hist.valid == ((1u << M) - 1u));
+      if (full) {
         // ---- steady state (full history, every pair usable): both loops fully
         //      unrolled, alpha_i in registers, no per-pair control flow ----
+        probe.set_steady();
         int idx = hist.mem_pos + MS - 1;
         idx = (idx >= MS) ? idx - MS : idx;
         T sv[E], yv[E];
@@ -524,14 +606,89 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
         }
       }
 
+      probe.mark(kPhRecursion);
       T alpha_init;
       const T dginit = lbfgs_direction<P>(rc, g, q, xx, hist, alpha_init);
+      probe.mark(kPhDirection);
       T xn[E], gn[E];
       T fn_val;
+      const uint32_t nfev_before = nfev;
       lbfgs_search<LS>(fn, ctx, rc, x, f, g, xn, fn_val, gn, alpha_init, q, dginit, nfev);
+      probe.search(!(dginit >= T(0)), nfev - nfev_before);
 
       const T prev_value = f;
       T x_delta, gnorm_inf, x_inf;
+      if constexpr (LbfgsPlan<Fn, M, kResume, LS>::kPlain) {
+        // ---- steady-state tail: the pair update and Progress::Update as one straight block behind ONE vote ----
+        // The pair sums, the three norms and the stopping tests read only the line search's result, so they are
+        // formed together, the norms' REDUX and the tests overlapping the sums' DMMA chain.  The block runs when the
+        // history was full and usable, the trial value is finite, the curvature bound accepts the pair outright, the
+        // plateau test (stop.past > 0) has its ring filled and either does not compare yet or its division-free bound
+        // says it does not fire, and no other stopping test fires; then it makes exactly the effects of the general
+        // path below, in the same order.  Otherwise it has made none and the general path runs.
+        T sd[E], yd[E];
+#pragma unroll
+        for (int j = 0; j < E; ++j) { sd[j] = xn[j] - x[j]; yd[j] = gn[j] - g[j]; }
+        T sy, ss, yy, xx_next;
+        warp_sum4_p<P, T, E>(lane_dot_p<P, T, E>(sd, yd), lane_dot_p<P, T, E>(sd, sd), lane_dot_p<P, T, E>(yd, yd),
+                             lane_dot_p<P, T, E>(xn, xn), rc, sy, ss, yy, xx_next);
+        maxabs3(rc, sd, gn, xn, x_delta, gnorm_inf, x_inf);
+        ProgressState<T> next = prog;
+        const int status =
+            progress_gradient_test(progress_update_head(next, stop, prev_value, fn_val, x_delta, gnorm_inf), next,
+                                   stop, x_inf);
+        // progress.h:280-298 (cno_progress.cuh): the plateau test's first bound, "does not fire"
+        const T past_f = ring[prog.ring_pos];
+        const T diff = cabs(past_f - fn_val), bound = stop.past_delta * smax(T(1), cabs(fn_val));
+        const bool past_quiet =
+            !(stop.past > 0) ||
+            (prog.ring_size == stop.past &&
+             ((int)next.num_iterations <= stop.past ||
+              (cfinite(diff) && cfinite(bound) && bound > T(0) && diff > T(2) * bound)));
+        if (uni(full && cfinite(fn_val) && curvature_surely_above_eps(sy, ss, yy) && past_quiet &&
+                status == CNO_STATUS_CONTINUE)) {
+          const T rho_new = T(1) / sy;
+          const int slot = hist.ring_slot();  // mem_count = M >= R
+          if constexpr (R > 0) {
+            SV::store(S + slot * SM::kVec, lane, rs[R - 1]);
+            SV::store(Y + slot * SM::kVec, lane, ry[R - 1]);
+          } else {
+            SV::store(S + slot * SM::kVec, lane, sd);
+            SV::store(Y + slot * SM::kVec, lane, yd);
+          }
+          __syncwarp();  // all lanes are done reading rho_s in this iteration's loops
+          if (lane == 0) rho_s[slot] = (R > 0) ? rrho[RA - 1] : rho_new;
+#pragma unroll
+          for (int j = R - 1; j > 0; --j) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) { rs[j][e] = rs[j - 1][e]; ry[j][e] = ry[j - 1][e]; }
+            rrho[j] = rrho[j - 1];
+          }
+          if constexpr (R > 0) {
+#pragma unroll
+            for (int e = 0; e < E; ++e) { rs[0][e] = sd[e]; ry[0][e] = yd[e]; }
+            rrho[0] = rho_new;
+          }
+          hist.record(sy);
+          lbfgs_update_gamma(gamma, sy, yy);
+#pragma unroll
+          for (int j = 0; j < E; ++j) { x[j] = xn[j]; g[j] = gn[j]; }
+          f = fn_val;
+          xx = xx_next;
+          __syncwarp();
+          if (stop.past > 0) {
+            if (lane == 0) ring[next.ring_pos] = fn_val;
+            next.ring_pos = (next.ring_pos + 1 == stop.past) ? 0 : next.ring_pos + 1;
+            __syncwarp();
+          }
+          prog = next;
+          prog.status = status;
+          local_it++;
+          probe.mark(kPhPairUpdate);
+          probe.end();
+          continue;
+        }
+      }
       if (uni(!cfinite(fn_val))) {
         // :239-241 return current: x, g, f unchanged; x_delta = |x - x|_inf (progress.h:190) is 0,
         // or NaN when x itself holds a non-finite component (rare path, computed as written).
@@ -574,6 +731,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
           hist.record(sy);
         }
         lbfgs_update_gamma(gamma, sy, yy);
+        probe.mark(kPhPairUpdate);
         // the norms Progress::Update and the next step need, then the next state
         maxabs3(rc, sd, gn, xn, x_delta, gnorm_inf, x_inf);
 #pragma unroll
@@ -587,7 +745,10 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
       if constexpr (kSecond) nfev++;  // its Hessian evaluation (progress.h:206-207; value unused, DESIGN.md)
       progress_update<T>(prog, stop, ring, lane, prev_value, f, x_delta, gnorm_inf, x_inf);
       local_it++;
-    } while (uni(prog.status == CNO_STATUS_CONTINUE && (!kResume || local_it < ra.max_iterations)));
+      probe.end();
+      if (!uni(prog.status == CNO_STATUS_CONTINUE && (!kResume || local_it < max_local_it))) break;
+    }
+    probe.stop();
 
     if constexpr (kResume) {
       if (uni(prog.status == CNO_STATUS_CONTINUE)) {
@@ -624,6 +785,7 @@ lbfgs_minimize_kernel(const Fn fn, const typename Fn::Scalar* __restrict__ x0,
 
     store_result<T, D>(out, b, lane, x, g, f, prog, nfev);
   }
+  probe.flush(lane);
   if constexpr (kHelpers > 0) {
     if (solver_warp) fn.release_helper(EvalCtx{lane, 0, stage_ptr, slot});
   }

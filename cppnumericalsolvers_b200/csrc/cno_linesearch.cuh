@@ -17,6 +17,16 @@
 
 namespace cno {
 
+#ifdef CNO_LBFGS_PHASE_CLOCKS
+// Phase probe of lbfgs_minimize_kernel (cno_lbfgs.cuh, measurement builds only): clock64() once the search's first
+// trial has been decided, one slot per warp of the CTA, written by lane 0.
+__shared__ long long cno_ls_first_trial_clock[32];
+#define CNO_LS_FIRST_TRIAL_CLOCK(nfev) \
+  if ((nfev) == 1 && (threadIdx.x & 31) == 0) cno_ls_first_trial_clock[threadIdx.x >> 5] = clock64()
+#else
+#define CNO_LS_FIRST_TRIAL_CLOCK(nfev)
+#endif
+
 template <class T>
 __device__ __forceinline__ T max_abs3(T x, T y, T z) {  // more_thuente.h:409-411
   return smax(cabs(x), smax(cabs(y), cabs(z)));
@@ -225,6 +235,7 @@ __device__ __forceinline__ int cvsrch(const Fn& fn, const Ctx& ctx, const RC& rc
     if (brackt & (stmax - stmin <= xtol * stmax)) info = 2;
     if ((f <= ftest1) & (cabs(dg) <= gtol * (-dginit))) info = 1;
 
+    CNO_LS_FIRST_TRIAL_CLOCK(nfev);
     if (uni(info != 0)) return nfev;  // :219
 
     if (stage1 & (f <= ftest1) & (dg >= smin(ftol, gtol) * dginit)) stage1 = false;

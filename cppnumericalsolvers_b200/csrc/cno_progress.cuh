@@ -42,11 +42,10 @@ __device__ __forceinline__ void progress_start(ProgressState<T>& p) {
   p.status = CNO_STATUS_NOT_STARTED;
 }
 
+// progress.h:153-277: the counters and the tests before the plateau test.  Returns the status they decide.
 template <class T>
-__device__ __forceinline__ void progress_update(ProgressState<T>& p, const StopParams<T>& stop,
-                                                T* __restrict__ ring, const int lane,
-                                                T prev_value, T cur_value, T x_delta,
-                                                T gradient_norm, T x_inf) {
+__device__ __forceinline__ int progress_update_head(ProgressState<T>& p, const StopParams<T>& stop, T prev_value,
+                                                    T cur_value, T x_delta, T gradient_norm) {
   p.num_iterations++;
   p.f_delta = cabs(cur_value - prev_value);
   p.x_delta = x_delta;
@@ -75,6 +74,26 @@ __device__ __forceinline__ void progress_update(ProgressState<T>& p, const StopP
       p.f_delta_violations = 0;
     }
   }
+  return status;
+}
+
+// progress.h:299-317: the gradient-norm test, when no earlier test has fired.
+template <class T>
+__device__ __forceinline__ int progress_gradient_test(int status, const ProgressState<T>& p, const StopParams<T>& stop,
+                                                      T x_inf) {
+  if (status == CNO_STATUS_CONTINUE && stop.gradient_norm > 0) {  // :299-317
+    const T scale = stop.gradient_norm_relative ? smax(T(1), x_inf) : T(1);
+    if (p.gradient_norm < stop.gradient_norm * scale) status = CNO_STATUS_GRADIENT_NORM_VIOLATION;
+  }
+  return status;
+}
+
+template <class T>
+__device__ __forceinline__ void progress_update(ProgressState<T>& p, const StopParams<T>& stop,
+                                                T* __restrict__ ring, const int lane,
+                                                T prev_value, T cur_value, T x_delta,
+                                                T gradient_norm, T x_inf) {
+  int status = progress_update_head(p, stop, prev_value, cur_value, x_delta, gradient_norm);
   if (uni(status == CNO_STATUS_CONTINUE && stop.past > 0)) {  // :280-298
     const int pp = stop.past;
     if (uni(p.ring_size != pp)) {
@@ -109,11 +128,7 @@ __device__ __forceinline__ void progress_update(ProgressState<T>& p, const StopP
       __syncwarp();
     }
   }
-  if (status == CNO_STATUS_CONTINUE && stop.gradient_norm > 0) {  // :299-317
-    const T scale = stop.gradient_norm_relative ? smax(T(1), x_inf) : T(1);
-    if (p.gradient_norm < stop.gradient_norm * scale) status = CNO_STATUS_GRADIENT_NORM_VIOLATION;
-  }
-  p.status = status;
+  p.status = progress_gradient_test(status, p, stop, x_inf);
 }
 
 // The scalars of instance b's result record, written by one thread: the returned FunctionState's value and Progress.
